@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the MAPDN var_voltage_control env step (BASELINE.json metric: env-steps/sec).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 Headline workload (BASELINE.json configs[1]): case33 (33-bus feeder), 4096 env instances per GPU, Bowl
 voltage barrier, noise on, synthetic load/PV profiles and random actions (the reference's data
@@ -22,6 +22,8 @@ obs inside the timed region). The same line carries
   `parity.reference_fixture`: the same device replaying a trajectory that the reference's own env code produced
   (tests/golden/ref_env_case33_bowl.npz);
 * `cpu_baseline`: the CPU arm timed on this box's usable cores (affinity + cgroup quota), with a 1-core rate.
+
+`--dump-outputs DIR`: the last timed headline step's reward / terminated / info / obs as DIR/<name>.npy (seeded inputs).
 
 `--impl reference` times the reference's CPU implementation of the path on the host cores: real pandapower
 (`import pandapower`, also looked up under baseline/_ref) when it is importable, else the oracle port
@@ -335,8 +337,26 @@ class Timer:
         return float(t.item())
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays, rank, world, limit=DUMP_LIMIT_BYTES):
+    """``arrays`` (env rows in dim 0) as ``out_dir/<name>.npy``; above ``limit`` bytes a seeded sample of rows + ``env_ids``."""
+    host = {k: v.detach().cpu().numpy() for k, v in arrays.items()}
+    host = {k: v.astype(np.float64 if v.dtype == np.float64 else np.float32) for k, v in host.items()}
+    B = next(iter(host.values())).shape[0]
+    row_bytes = sum(v.nbytes for v in host.values()) / max(1, B)
+    if row_bytes * B > limit:
+        keep = np.sort(np.random.default_rng(0).choice(B, int(limit // (row_bytes + 8)), replace=False))
+        host = {k: v[keep] for k, v in host.items()}
+        host["env_ids"] = keep.astype(np.float64)
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in host.items():
+        np.save(os.path.join(out_dir, (k if world == 1 else f"{k}_rank{rank}") + ".npy"), v)
+
+
 def measure(sc, barrier, global_batch, K, W, Ke, tm, local, rank, flush, lanes=0, clocks=None, obs_dtypes=("f64",),
-            min_warm=0):
+            min_warm=0, dump_dir=None):
     """Device-timed and end-to-end throughput of one configuration, sharded over the ranks of this job."""
     import torch
     from mapdn_b200 import cases
@@ -388,6 +408,9 @@ def measure(sc, barrier, global_batch, K, W, Ke, tm, local, rank, flush, lanes=0
     w1 = time.perf_counter()
     launches = env.launch_count - launches0
     clk = clocks.stop(w0, w1, t_load0) if clocks is not None else None
+    if dump_dir:
+        dump_outputs(dump_dir, dict(reward=env.reward, terminated=env.terminated, info=env.info, obs=env.obs), rank,
+                     tm.world)
     dev_ms = tm.max_over_ranks(sum(a.elapsed_time(b) for a, b in zip(ev0, ev1)))
     assert returns.shape[0] == global_batch and bool(torch.isfinite(returns).all())
     # side metrics of the last timed step (SURVEY §8d): Newton iterations per solve, diverged fraction
@@ -452,7 +475,7 @@ def roofline_of(m, peak, peak_src, traffic=None, ncu=None):
     ms = m["ms_per_step"]
     achieved = m["_alg_bytes_per_launch"] / (ms * 1e-3) / 1e9
     return dict(bound="hbm", achieved=achieved, peak=peak, unit="GB/s", frac=achieved / peak, traffic=traffic,
-                peak_source=f"{peak_src} (MEASURED_PEAKS.json hbm_gbs)" if peak_src == "measured" else "fallback 6.65 TB/s",
+                peak_source=f"{peak_src} (MEASURED_PEAKS.json hbm_gbs)" if peak_src == "measured" else "fallback 3.35 TB/s",
                 kernel=f"env_kernel<{m['lanes_per_env']},STEP>", algorithmic_bytes_per_launch=m["_alg_bytes_per_launch"],
                 ncu=ncu,
                 binding_bound="dependent-instruction latency of the slowest env of the launch (5 Newton iterations), fp64 issue "
@@ -578,7 +601,7 @@ def run_ours(args):
     B = args.batch or {"case33": 4096, "case141": 2048, "case322": 1024}[sc]
     custom = bool(args.scenario or args.batch or args.barrier or args.lanes)
     K, W = args.steps, args.warmup
-    flush = None if args.no_flush else torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = None if args.no_flush else torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > the H100's 50 MB L2
     Ke = max(3, min(K, args.e2e_steps))
 
     parity = None
@@ -586,12 +609,13 @@ def run_ours(args):
         parity = parity_check(sc, barrier, B, local)
     clocks = ClockSampler(local) if rank == 0 else None
     m = measure(sc, barrier, B * world, K, W, Ke, tm, local, rank, flush, lanes=args.lanes, clocks=clocks,
-                obs_dtypes=("f64", "f32", "staged", "compact_f64", "compact_f32", "compact_zc_f64"), min_warm=50)
+                obs_dtypes=("f64", "f32", "staged", "compact_f64", "compact_f32", "compact_zc_f64"), min_warm=50,
+                dump_dir=args.dump_outputs)
 
     # ---- the other BASELINE.json configurations of this GPU count ----
     subs = []
     if not custom and not args.no_sub:
-        Ks, Ws = max(10, min(K, 50)), 5
+        Ks, Ws = K, 5
         plan = []
         for cid, c in CONFIGS.items():
             if cid == HEADLINE:
@@ -617,7 +641,7 @@ def run_ours(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         peak, peak_src = float(peaks["hbm_gbs"]), "measured"
     except Exception:
-        peak = 6650.0
+        peak = 3350.0
     traffic = {}
     try:
         traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
@@ -649,6 +673,7 @@ def run_ours(args):
                             n_bus=net.n_bus, n_agents=net.n_sgen, obs_dim=m["obs_dim"], global_batch=B * world,
                             lanes_per_env=m["lanes_per_env"], envs_per_block=m["envs_per_block"],
                             parallelism=f"envs sharded over {world} GPU(s)", numa=numa,
+                            gpu=torch.cuda.get_device_name(local),
                             warmup_steps_done=m["warmup_steps_done"],
                             l2="flushed between steps (256 MiB memset, outside the event pairs)" if flush is not None
                             else "not flushed", timing="sum of per-step CUDA-event pairs, max over ranks"),
@@ -689,7 +714,11 @@ def main():
     ap.add_argument("--cpu-sample", type=int, default=0)
     ap.add_argument("--cpu-cores", type=int, default=0)
     ap.add_argument("--e2e-steps", type=int, default=50)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step of the headline configuration returned as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.warmup < 3:
         args.warmup = 3
     return run_reference(args) if args.impl == "reference" else run_ours(args)

@@ -1,5 +1,5 @@
 /*
- * mapdn_b200.h - C-ABI of the B200-native batched MAPDN voltage-control environment step.
+ * mapdn_b200.h - C-ABI of the H100-native batched MAPDN voltage-control environment step.
  *
  * The reference (Future-Power-Networks/MAPDN) has no FFI: the hot path sits behind the Python
  * class VoltageControl(MultiAgentEnv) (environments/var_voltage_control/voltage_control_env.py)
@@ -214,10 +214,9 @@ mapdn_status mapdn_wait(mapdn_env* env, void* stream);
  * longest one (:270-274); here the host receives obs_host [B, row_len] (double, or float when obs_is_f32) in which agent a
  * owns entries [agent_off[a], agent_off[a] + agent_len[a]) - its reference row without the padding (row_len = sum of
  * the lengths, rounded up to a multiple of 4 with zeros). The kernel writes the compact rows into device memory and ONE
- * contiguous copy-engine transfer moves them (measured 55 GB/s, against 37 GB/s for the kernel's own posted writes of
- * mapdn_step_host_pinned); actions are read from and reward / terminated / info written to host memory directly. All
+ * contiguous copy-engine transfer moves them (long contiguous rows are what the copy engine moves fastest); actions are read from and reward / terminated / info written to host memory directly. All
  * host buffers must be page-locked. direct = 1: the kernel writes the compact rows to obs_host itself instead (no
- * device staging, no copy; contiguous rows reach 43 GB/s, measured 5 % slower end to end than the copy). sync as in
+ * device staging, no copy; on an H100 about as fast end to end as the copy). sync as in
  * mapdn_step_host_pinned.
  */
 mapdn_status mapdn_obs_compact_layout(const mapdn_env* env, int32_t* agent_off /*[n_agents]*/,

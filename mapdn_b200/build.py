@@ -1,4 +1,4 @@
-"""Builds the C-ABI shared library ``mapdn_b200/libmapdn_b200.so`` in-tree with nvcc for sm_100a.
+"""Builds the C-ABI shared library ``mapdn_b200/libmapdn_b200.so`` in-tree with nvcc for sm_90a.
 
     python -m mapdn_b200.build [--force]
 
@@ -20,7 +20,7 @@ DEPS = SOURCES + [os.path.join(CSRC, f) for f in ("env_kernel.cuh", "kernel_para
     os.path.join(HERE, "..", "include", "mapdn_b200.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--shared", "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr",
 ]
 

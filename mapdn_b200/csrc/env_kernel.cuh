@@ -1,4 +1,4 @@
-// Fused batched environment kernel for sm_100a: action clip -> bus injections -> polar
+// Fused batched environment kernel for sm_90a: action clip -> bus injections -> polar
 // Newton-Raphson on the (radial) Ybus with a zero-fill 2x2-block elimination -> reward / info ->
 // next profile row (+ noise) -> zone-masked observation gather. One launch per env step.
 //
@@ -454,7 +454,7 @@ __device__ __forceinline__ bool nr_solve(const Params& p, const Hot& h, const Sl
         if (fl & kEschedLeaf) { p01 = make_double2(0.0, 0.0); p23 = p01; pt = p01; }     // a lane starting a new chain
         if (fl & kEschedLoad0) { const double2* k0 = s.node(c0); p01 = k0[A_UP]; p23 = k0[A_DN]; pt = k0[A_T]; }
         d01.x -= p01.x; d01.y -= p01.y; d23.x -= p23.x; d23.y -= p23.y; r.x -= pt.x; r.y -= pt.y;
-        const Own own_next = load_own(ed_next);          // not touched before its own step (measured: -2.5 % behind the child loads)
+        const Own own_next = load_own(ed_next);          // not touched before its own step: issued behind the child loads
         if (fl & kEschedLoad1) {                          // child 1 (branching buses only): always shared memory
           const double2* k1 = s.node(c1);
           const double2 q01 = k1[A_UP], q23 = k1[A_DN], qt = k1[A_T];
@@ -612,7 +612,7 @@ __device__ __forceinline__ bool nr_solve(const Params& p, const Hot& h, const Sl
     }
     PROF(6)
     // --- update (theta += dtheta, V += V * dV/V) and V = Vm exp(j theta): a pass of its own - inside the back sweep the
-    //     sin/cos chain would sit in front of the next step of the in-order warp (measured: +200 cycles per step) ---
+    //     sin/cos chain would sit in front of the next step of the in-order warp ---
 #pragma unroll 4
     for (int i = gl; i < npq; i += G) {
       if (!done) {
@@ -1005,7 +1005,7 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
       }
       // (droop re-stages the loads every round: the staging area is overwritten by the Newton iteration)
       // Written once, instantiated for the two staging places (block-uniform choice): a branch per access inside the
-      // loops cost 0.7 us per step on case33.
+      // loops would cost time in every step.
       auto stage_and_gather = [&](auto stg) {
 #pragma unroll 4
         for (int l = gl; l < nl; l += G) {

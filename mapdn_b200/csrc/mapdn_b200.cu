@@ -213,7 +213,7 @@ std::vector<T> vec_or(const T* p, size_t n, T fill) {
 }
 
 using KernelFn = void (*)(const Params);
-constexpr int kHelperPairsPerWarp = 256;   // Box-Muller pairs of a CTA round per helper warp (1024 measured slower: +2 us on case33)
+constexpr int kHelperPairsPerWarp = 256;   // Box-Muller pairs of a CTA round per helper warp
 
 template <int G>
 KernelFn kernel_for_mode(int mode) {
@@ -493,8 +493,8 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
   for (int l = 0; l < n_lev; ++l) max_width = std::max(max_width, elev[l + 1] - elev[l]);
   for (int i = 0; i < npq; ++i) max_children = std::max(max_children, nchild[i]);
   int G = cfg->lanes_per_env;
-  if (G == 0) G = (npq <= 64) ? 8 : (npq <= 256 ? 32 : 64);      // measured on B200 (profiles/r02_sweeps.txt)
-  if (meshed) G = 32;                    // the dense fallback works one warp per env     // measured on B200: 8 lanes/env for 33-bus feeders, a full warp beyond
+  if (G == 0) G = (npq <= 64) ? 8 : (npq <= 256 ? 32 : 64);      // fastest on H100 at every BASELINE size (DESIGN.md §4)
+  if (meshed) G = 32;                    // the dense fallback works one warp per env
   // Flat schedules for this G: a level wider than G takes several steps; idle lanes get the trash record.
   // Lanes follow chains: a bus is placed on the lane that handled its child (forward sweep) / its parent
   // (back sweep) in the immediately preceding step whenever that lane is free, so the dependent value can
@@ -937,10 +937,10 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
   const int n_sm = dp.multiProcessorCount;
   int stride2 = 0, epb = 0;
   bool stage_rec = false;
-  // Two ways to buy shared memory when it limits the envs per SM, both with a price (measured, profiles/): (a) the four
+  // Two ways to buy shared memory when it limits the envs per SM, both with a price: (a) the four
   // once-per-step tables (Y[i,slack], obs program, line tables) stay in global memory instead of the staged blob - their
   // first touch after an L2 flush is an HBM round trip at the start of the epilogue, softened by an L2 prefetch at kernel
-  // start; (b) the prologue stages the scaled loads inside the node records - index arithmetic, +1.3 k cycles per step on
+  // start; (b) the prologue stages the scaled loads inside the node records - index arithmetic in every step of
   // case33. Each is used only if it lets the batch finish in fewer rounds (case322 x 1024: 4 envs per SM and 2 rounds
   // instead of 3 and 3).
   struct Plan { bool cold, rec, ok; int st2, epb; long long rounds; };
@@ -951,13 +951,12 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
     Plan pl{cold, rec, false, 0, 0, 0};
     if (rec && !stage_fits_records(npq, nl)) return pl;
     pl.st2 = env_stride2_for(npq, ng, nl, G, rec);
-    // measured on B200 (profiles/): two solver warps per CTA for small sub-warp groups, four for one-warp envs,
+    // two solver warps per CTA for small sub-warp groups, four for one-warp envs,
     // as many multi-warp envs as fit (<= 512 solver threads)
     int c_epb = (G <= 16) ? 2 * unit : 4 * unit;
     if (G > 32) while (c_epb > 1 && c_epb * G > 512) --c_epb;
     // Few-round batches (the BASELINE.json configs): one CTA per SM holding ceil(B / (SMs * rounds)) envs balances the
-    // SMs exactly (case33 x 4096: 147 CTAs of 28 envs instead of 512 of 8, i.e. 7 instead of up to 8 solver warps on
-    // the busiest SM; case141 x 2048: 2 rounds of 7). Many-round batches keep several small CTAs per SM.
+    // SMs exactly (case33 x 4096 on 132 SMs: 128 CTAs of 32 envs). Many-round batches keep several small CTAs per SM.
     auto fits = [&](int c) { return smem_with(cold, pl.st2, c) <= max_smem && c * G <= (G <= 32 ? 256 : 512); };
     for (int r = 1; r <= 3; ++r) {
       int c = (cfg->batch + n_sm * r - 1) / (n_sm * r);
@@ -991,7 +990,7 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
   e->dense = meshed;
   e->G = G; e->threads = epb * G; e->epb = epb; e->smem = static_cast<int>(smem_for(epb));
   {   // helper warps (next profile rows + noise, concurrent with the Newton iteration): one per 256 Box-Muller pairs of a
-      // CTA round, at most 4 -- a single warp was the critical path of case322 (197 -> 169 us with two)
+      // CTA round, at most 4 -- a single warp can be the critical path of case322
     const int n_pair = (ng + 2 * nl + 1) / 2;
     e->helper_threads = 32 * std::min(4, std::max(1, (epb * n_pair + kHelperPairsPerWarp - 1) / kHelperPairsPerWarp));
   }

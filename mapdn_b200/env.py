@@ -235,7 +235,8 @@ class BatchedVoltageControl:
         zero padding of the reference's ``get_obs`` - agent ``a`` owns ``obs[:, off:off + n]`` with ``(off, n) =
         self.obs_slices[a]`` (a strided NumPy view, no copy; :meth:`expand_obs` rebuilds the padded array). The rows
         go through device memory and ONE contiguous copy-engine transfer by default (``staged=False`` makes the kernel
-        write them to host memory itself, like the padded path: measured 5 % slower)."""
+        write them to host memory itself, like the padded path: on an H100 about as fast, 18.7 against 18.8 M
+        env-steps/s for case33 x 4096)."""
         hb = self._host_buffers()
         hb["actions"].numpy()[...] = actions
         f32 = np.dtype(obs_dtype) == np.float32

@@ -131,6 +131,12 @@ def fixture_path(root, name):
     return os.path.join(root, "tests", "golden", f"ref_env_{name}.npz")
 
 
+def digest(a):
+    """SHA-256 of an array's float64 values: exact equality against a fixture without storing the array."""
+    import hashlib
+    return hashlib.sha256(np.ascontiguousarray(a, dtype=np.float64).tobytes()).hexdigest()
+
+
 def n_steps_of(sc):
     return sum(1 for op in sc["ops"] if op[0] == "step")
 

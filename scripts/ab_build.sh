@@ -12,7 +12,7 @@ mkdir -p scripts/variants
 for spec in "$@"; do
   name="${spec%%=*}"; flags="${spec#*=}"
   echo "building scripts/variants/$name.so with: $flags"
-  nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 --shared -Xcompiler -fPIC \
+  nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 --shared -Xcompiler -fPIC \
        --expt-relaxed-constexpr $flags -o scripts/variants/$name.so mapdn_b200/csrc/mapdn_b200.cu &
 done
 wait

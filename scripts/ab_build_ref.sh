@@ -18,7 +18,7 @@ for f in ("include/mapdn_b200.h", "mapdn_b200/csrc/mapdn_b200.cu"):
     open(f"{t}/{f}", "w").write(s)
 PY
 mkdir -p scripts/variants
-nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 --shared -Xcompiler -fPIC --expt-relaxed-constexpr \
+nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 --shared -Xcompiler -fPIC --expt-relaxed-constexpr \
      $flags -o scripts/variants/$name.so "$tmp/mapdn_b200/csrc/mapdn_b200.cu"
 rm -rf "$tmp"
 ls -la scripts/variants/$name.so

@@ -1,6 +1,6 @@
 // Probe (not part of the product): bandwidth of a kernel's own stores into pinned host memory (posted PCIe writes) for
 // different store shapes. 4096 rows of 1600 bytes (case33 observations without padding) per launch.
-//   nvcc -O2 -gencode arch=compute_100a,code=sm_100a -o scripts/probes/posted_write_probe scripts/probes/posted_write_probe.cu
+//   nvcc -O2 -gencode arch=compute_90a,code=sm_90a -o scripts/probes/posted_write_probe scripts/probes/posted_write_probe.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #define CK(x) do { cudaError_t e = (x); if (e != cudaSuccess) { printf("%s: %s\n", #x, cudaGetErrorString(e)); return 1; } } while (0)
@@ -42,7 +42,7 @@ int main() {
   CK(cudaMallocHost(&host, bytes)); CK(cudaMalloc(&dev, bytes));
   cudaEvent_t e0, e1; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
   const int reps = 30;
-  for (int blocks : {148, 296, 592}) {
+  for (int blocks : {132, 264, 528}) {
     const int rpb = (ROWS + blocks - 1) / blocks;
     for (int mode = 0; mode < 4; ++mode) {
       for (int tgt = 0; tgt < 2; ++tgt) {

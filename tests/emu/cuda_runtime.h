@@ -79,10 +79,10 @@ static inline cudaError_t cudaMemsetAsync(void* d, int v, size_t n, cudaStream_t
 static inline cudaError_t cudaPointerGetAttributes(cudaPointerAttributes* a, const void* p) {   // every host buffer counts as pinned
   a->type = cudaMemoryTypeHost; a->device = 0; a->devicePointer = const_cast<void*>(p); a->hostPointer = const_cast<void*>(p); return cudaSuccess;
 }
-static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp* p, int) {                      // the B200 numbers the host code plans with
-  memset(p, 0, sizeof(*p)); snprintf(p->name, sizeof(p->name), "emulated B200");
-  p->multiProcessorCount = 148; p->sharedMemPerBlockOptin = 232448; p->sharedMemPerMultiprocessor = 233472; p->reservedSharedMemPerBlock = 1024;
-  p->major = 10; p->minor = 0; p->totalGlobalMem = size_t(180) << 30; p->maxThreadsPerMultiProcessor = 2048; p->regsPerMultiprocessor = 65536;
+static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp* p, int) {                      // the H100 SXM numbers the host code plans with
+  memset(p, 0, sizeof(*p)); snprintf(p->name, sizeof(p->name), "emulated H100");
+  p->multiProcessorCount = 132; p->sharedMemPerBlockOptin = 232448; p->sharedMemPerMultiprocessor = 233472; p->reservedSharedMemPerBlock = 1024;
+  p->major = 9; p->minor = 0; p->totalGlobalMem = size_t(80) << 30; p->maxThreadsPerMultiProcessor = 2048; p->regsPerMultiprocessor = 65536;
   p->sharedMemPerBlock = 49152; p->warpSize = 32; return cudaSuccess;
 }
 template <class F> static inline cudaError_t cudaFuncSetAttribute(F, cudaFuncAttribute, int) { return cudaSuccess; }

@@ -24,7 +24,7 @@ def test_configs_are_the_baseline_json_configs():
         c = bench.CONFIGS[cid]
         assert c["scenario"] in txt and str(c["batch"]) in txt
         assert re.search(c["barrier"], txt, re.I)
-        assert f"{c['n_gpus']}×B200" in txt or f"{c['n_gpus']}xB200" in txt
+        assert f"{c['n_gpus']}×H100" in txt or f"{c['n_gpus']}xH100" in txt
     assert bench.CONFIGS[bench.HEADLINE]["scenario"] == "case33" and bench.CONFIGS[bench.HEADLINE]["batch"] == 4096
 
 
@@ -87,3 +87,4 @@ def test_reference_fixture_leg_of_the_parity_record():
         rec = bench.reference_fixture_check(0, name=name, make_env=Standin)
         assert rec["n_steps"] >= 6 and rec["max_abs_dreward"] < 1e-11 and rec["max_abs_dinfo"] < 1e-11
         assert rec["max_abs_dobs"] < 1e-11 and rec["max_abs_dstate"] < 1e-9
+

@@ -1,4 +1,4 @@
-"""The C-ABI library builds for sm_100a (nvcc cross-compiles on the CPU box), loads, and exports
+"""The C-ABI library builds for sm_90a (nvcc cross-compiles on the CPU box), loads, and exports
 every entry point declared in include/mapdn_b200.h. No compute calls - no GPU needed."""
 import ctypes
 import os
@@ -103,16 +103,16 @@ def test_create_validates_arguments_without_touching_the_gpu(built_lib):
 
 
 def test_product_library_is_the_device_build_not_the_cpu_emulation(built_lib):
-    """The shipped library is the nvcc build: it carries sm_100a device code and none of the emulation's symbols; the
+    """The shipped library is the nvcc build: it carries sm_90a device code and none of the emulation's symbols; the
     product's loader and build script know nothing of tests/emu (the CPU SIMT emulation is test infrastructure)."""
     import subprocess
     from mapdn_b200 import build
-    assert "-DMAPDN_HOST_EMU" not in " ".join(build.NVCC_FLAGS) and any("sm_100a" in f for f in build.NVCC_FLAGS)
+    assert "-DMAPDN_HOST_EMU" not in " ".join(build.NVCC_FLAGS) and any("sm_90a" in f for f in build.NVCC_FLAGS)
     syms = subprocess.run(["nm", "-DC", built_lib], capture_output=True, text=True).stdout
     assert "emu::" not in syms and "launch_impl" not in syms
     elf = subprocess.run(["cuobjdump", "-lelf", built_lib], capture_output=True, text=True)
     if elf.returncode == 0:
-        assert "sm_100a" in elf.stdout
+        assert "sm_90a" in elf.stdout
     for f in ("_capi.py", "build.py", "env.py"):
         src = open(os.path.join(ROOT, "mapdn_b200", f)).read()
         assert "emu" not in src.replace("enumerate", "") or f == "env.py" and "tests/emu" not in src

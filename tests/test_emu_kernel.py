@@ -2,7 +2,7 @@
 tests/emu/cuda_runtime.h - a SIMT emulation with one OS thread per CUDA thread, counting barriers for
 __syncthreads / bar.sync / bar.arrive / bar.red, exchange arrays for __shfl / __ballot - and executed against the oracle
 and against the reference-executed fixtures. It proves the kernel's LOGIC (schedules, lock-step groups, multi-warp
-groups, helper warps, RNG, epilogue) without a GPU; the `-m gpu` tests prove the sm_100a build. The emulated library is
+groups, helper warps, RNG, epilogue) without a GPU; the `-m gpu` tests prove the sm_90a build. The emulated library is
 test infrastructure: the product never loads it, and the device build is byte-identical with or without the
 MAPDN_HOST_EMU guards (same SASS)."""
 import json

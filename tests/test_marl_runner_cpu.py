@@ -1,18 +1,30 @@
 """The batched runner feeds the REFERENCE's own learner code (models/maddpg.py, utilities/trainer.py) unchanged.
 
-Runs where /root/reference exists (this container; it is imported in the test only, never by the product) on a CPU
-stand-in for BatchedVoltageControl; skipped on the GPU box. The GPU leg with the real env and an in-repo model of the
-same interface is tests/test_gpu_extras.py::test_marl_runner_on_device."""
+The learners are not part of this repository: scripts/make_marl_golden.py ran these cases with them and recorded every
+call of the runner (tests/golden/marl_replay.npz); :class:`ReplayNet` answers with the recorded outputs after checking the
+runner asked the same, and updates check the batches handed to the trainer. The GPU leg with the real env and an in-repo
+model of the same interface is tests/test_gpu_round2.py::test_marl_runner_on_device."""
+import json
 import os
 import sys
 from collections import namedtuple
+from types import SimpleNamespace
 
 import numpy as np
 import pytest
 import torch
 
-REF = "/root/reference"
-pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "models")), reason="reference tree not present")
+from conftest import ROOT
+from oracle.ref_scenarios import digest
+
+REF = os.environ.get("MAPDN_REFERENCE_ROOT", "")      # only the recording script runs the reference
+GOLDEN = os.path.join(ROOT, "tests", "golden", "marl_replay.npz")
+ALGS = ["iddpg", "maddpg", "matd3", "sqddpg", "facmaddpg", "mappo", "ippo", "coma"]
+B, N, OD, T = 5, 3, 7, 6                     # stand-in env: batch, agents, obs dim, max_steps
+
+
+def dig(t):
+    return digest(t.detach().cpu().numpy())
 
 
 class FakeBatchedEnv:
@@ -45,7 +57,6 @@ class FakeBatchedEnv:
         return reward, done, info
 
 
-@pytest.fixture
 def reference_on_path():
     """The reference imports its agents lazily (models/model.py:150-163) from namespace packages (no __init__.py); an
     unrelated `agents` distribution in site-packages would shadow them, so the reference's directories are registered
@@ -68,38 +79,107 @@ def reference_on_path():
             sys.modules[k] = v
 
 
-def _reference_maddpg(n_agents, obs_dim, max_steps):
+def _reference_trainer(alg, n_agents, obs_dim, max_steps):
     import yaml
-    from models.maddpg import MADDPG
+    from models.model_registry import Model as REGISTRY
     from utilities.trainer import PGTrainer
     d = yaml.safe_load(open(os.path.join(REF, "args", "default.yaml")))
-    d.update(yaml.safe_load(open(os.path.join(REF, "args", "alg_args", "maddpg.yaml")))["alg_args"])
+    d.update(yaml.safe_load(open(os.path.join(REF, "args", "alg_args", alg + ".yaml")))["alg_args"])
     d.update(agent_num=n_agents, obs_size=obs_dim, action_dim=1, cuda=False, max_steps=max_steps, action_scale=0.8,
-             action_bias=0.0, batch_size=8)
+             action_bias=0.0, batch_size=8, hid_size=8)
     args = namedtuple("Args", d.keys())(**d)
-    trainer = PGTrainer(args, MADDPG, env=None, logger=None)
-    return args, trainer
+    return args, PGTrainer(args, REGISTRY[alg], env=None, logger=None)
 
 
-def test_reference_maddpg_learns_from_device_batches(reference_on_path):
-    from mapdn_b200.marl_runner import BatchedMarlRunner, DeviceTransitionBuffer, attach
-    B, n, od, T = 5, 3, 7, 6
-    args, trainer = _reference_maddpg(n, od, max_steps=T)
-    net = attach(trainer.behaviour_net)
-    env = FakeBatchedEnv(B, n, od, episode_limit=4)
-    buf = DeviceTransitionBuffer(32, B, n, od, act_dim=1, hid_dim=args.hid_size, device=env.device)
+TRAIN_ENV = dict(voltage_barrier_type="bowl", action_scale=0.8, action_bias=0.0, seed=21)     # the train_process case
+
+
+def oracle_env():
+    from mapdn_b200 import cases
+    net, prof = cases.make_case("case33"), cases.make_profiles("case33", n_days=4)
+    return OracleBatchedEnv(net, prof, TRAIN_ENV, batch=1)
+
+
+def batch_digests(batch):
+    return [dig(x) for x in batch.unpacked()]
+
+
+def window_generator(k):                       # seeded windows: the k-th update's batch is reproducible
+    return torch.Generator().manual_seed(1000 + k)
+
+
+ARG_KEYS = ("max_steps", "action_scale", "action_bias", "hid_size", "batch_size", "num_eval_episodes")
+
+
+class ReplayNet:
+    """Answers the runner's calls as the reference learner did when the case was recorded."""
+
+    def __init__(self, g, case):
+        self.g, self.case = g, case
+        self.meta = json.loads(str(g[f"{case}/meta"]))
+        self.args = SimpleNamespace(**self.meta["args"])
+        init = torch.tensor(g[f"{case}/init_hidden"])
+        self.policy_dicts = [SimpleNamespace(init_hidden=lambda: init.clone())]
+        self.outputs = torch.tensor(g[f"{case}/outputs"])
+        self.i = self.pos = 0
+
+    def _answer(self, name, inputs, extra):
+        c = self.meta["calls"][self.i]
+        assert c["name"] == name and c["extra"] == extra, (self.i, name, c["name"])
+        assert c["in"] == [dig(x) for x in inputs], f"call {self.i} ({name}): the runner passed other inputs"
+        out = []
+        for shape in c["out"]:
+            n = 0 if shape is None else int(np.prod(shape))
+            out.append(None if shape is None else self.outputs[self.pos:self.pos + n].reshape(shape).clone())
+            self.pos += n
+        self.i += 1
+        return out
+
+    def get_actions(self, state, status, exploration, actions_avail, target, last_hid):
+        a, a_pol, lp, hid = self._answer("get_actions", [state, last_hid, actions_avail], [status, exploration, target])
+        return a, a_pol, lp, None, hid
+
+    def value(self, obs, act):
+        return self._answer("value", [obs, act], [])[0]
+
+    def finished(self):
+        return self.i == len(self.meta["calls"]) and self.pos == len(self.outputs)
+
+
+def _golden():
+    return np.load(GOLDEN)
+
+
+def _replay_on_stand_in(case):
+    from mapdn_b200.marl_runner import BatchedMarlRunner, DeviceTransitionBuffer
+    g = _golden()
+    net = ReplayNet(g, case)
+    env = FakeBatchedEnv(B, N, OD, episode_limit=4)
+    buf = DeviceTransitionBuffer(32, B, N, OD, act_dim=1, hid_dim=net.args.hid_size, device=env.device)
+    want = net.meta["update_batches"]
     updates = []
 
-    def update(runner, stat):                      # the reference's own optimisation steps on a device batch
-        if len(runner.buffer) >= 2 * args.batch_size:
-            batch = runner.buffer.get_batch(args.batch_size, n_windows=2)
-            w0 = [p.detach().clone() for p in trainer.behaviour_net.value_dicts.parameters()]
-            trainer.value_transition_process(stat, batch)
-            trainer.policy_transition_process(stat, batch)
-            updates.append(any(not torch.equal(a, b) for a, b in
-                               zip(w0, trainer.behaviour_net.value_dicts.parameters())))
+    def update(runner, stat):
+        if len(runner.buffer) >= 2 * net.args.batch_size:
+            k = len(updates)
+            batch = runner.buffer.get_batch(net.args.batch_size, n_windows=2, generator=window_generator(k))
+            updates.append(batch_digests(batch) == want[k])
     runner = BatchedMarlRunner(env, net, buf, update_fn=update)
     stat = runner.train_process({})
+    assert len(updates) == len(want) and updates and all(updates)
+    for k, v in net.meta["train_stat"].items():
+        assert abs(stat[k] - v) < 1e-12, k
+    ev = runner.evaluation({}, num_eval_episodes=B)
+    assert dig(torch.stack(env.actions_seen)) == net.meta["actions_seen"]          # training and evaluation steps
+    for k, v in net.meta["eval_stat"].items():
+        assert abs(ev[k] - v) < 1e-12, k
+    assert net.finished()
+    return runner, env, buf, stat, ev
+
+
+def test_reference_maddpg_learns_from_device_batches():
+    runner, env, buf, stat, ev = _replay_on_stand_in("maddpg_learns")
+    args, n, od = runner.args, N, OD
     assert runner.steps == T * B and buf.count == T
     # translate_action (utilities/util.py:123-132): every action the env saw lies inside [bias - scale, bias + scale]
     a = torch.stack(env.actions_seen)
@@ -117,55 +197,22 @@ def test_reference_maddpg_learns_from_device_batches(reference_on_path):
     assert float(lh.view(T, B, n, -1)[3].abs().max()) == 0.0 and float(lh.view(T, B, n, -1)[1].abs().max()) > 0.0
     # mean_train_* (model.py:243-261): info k is the constant k in the stand-in env
     assert abs(stat["mean_train_total_line_loss"] - 8.0) < 1e-12 and "mean_train_reward" in stat
-    assert updates and all(updates) and "mean_train_value_loss" in stat and np.isfinite(stat["mean_train_value_loss"])
-    ev = runner.evaluation({}, num_eval_episodes=B)
     assert abs(ev["mean_test_destroy"] - 10.0) < 1e-12 and np.isfinite(ev["mean_test_reward"])
 
 
-def _reference_trainer(alg, n_agents, obs_dim, max_steps):
-    import yaml
-    from models.model_registry import Model as REGISTRY
-    from utilities.trainer import PGTrainer
-    d = yaml.safe_load(open(os.path.join(REF, "args", "default.yaml")))
-    d.update(yaml.safe_load(open(os.path.join(REF, "args", "alg_args", alg + ".yaml")))["alg_args"])
-    d.update(agent_num=n_agents, obs_size=obs_dim, action_dim=1, cuda=False, max_steps=max_steps, action_scale=0.8,
-             action_bias=0.0, batch_size=8)
-    args = namedtuple("Args", d.keys())(**d)
-    return args, PGTrainer(args, REGISTRY[alg], env=None, logger=None)
-
-
 @pytest.mark.parametrize("alg", ["iddpg", "maddpg", "matd3", "sqddpg", "facmaddpg", "mappo", "ippo", "coma"])
-def test_reference_algorithms_run_unchanged_on_device_batches(reference_on_path, alg):
+def test_reference_algorithms_run_unchanged_on_device_batches(alg):
     """Eight of the ten algorithms of the reference's registry (models/model_registry.py) collect experience through the
     batched runner and run their own get_loss / optimiser steps on the device batches: deterministic and Gaussian
     policies, twin critics (MATD3: value width 2), coalition sampling (SQDDPG: value width sample_size), a mixer
-    (FACMADDPG), PPO / COMA advantage code. Not covered, for reasons upstream: IAC (`self.cuda_` is never set:
+    (FACMADDPG), PPO / COMA advantage code - replayed: the runner asks each learner what it asked then and hands its
+    trainer the same batches. Not covered, for reasons upstream: IAC (`self.cuda_` is never set:
     models/iac.py:90 raises AttributeError with the reference's own env too) and MAAC (its value() returns a
     concatenation that is not [batch, n, k]-shaped, models/maac.py:47-66)."""
-    from mapdn_b200.marl_runner import BatchedMarlRunner, DeviceTransitionBuffer, attach
-    B, n, od, T = 5, 3, 7, 6
-    args, trainer = _reference_trainer(alg, n, od, max_steps=T)
-    net = attach(trainer.behaviour_net)
-    env = FakeBatchedEnv(B, n, od, episode_limit=4)
-    buf = DeviceTransitionBuffer(32, B, n, od, act_dim=1, hid_dim=args.hid_size, device=env.device)
-    updates = []
-
-    def update(runner, stat):
-        if len(runner.buffer) >= 2 * args.batch_size:
-            batch = runner.buffer.get_batch(args.batch_size, n_windows=2)
-            w0 = [p.detach().clone() for p in trainer.behaviour_net.policy_dicts.parameters()]
-            trainer.value_transition_process(stat, batch)
-            trainer.policy_transition_process(stat, batch)
-            if args.mixer:
-                trainer.mixer_transition_process(stat, batch)
-            updates.append(any(not torch.equal(a, b) for a, b in zip(w0, trainer.behaviour_net.policy_dicts.parameters())))
-    runner = BatchedMarlRunner(env, net, buf, update_fn=update)
-    stat = runner.train_process({})
-    assert runner.steps == T * B and updates and all(updates)
-    assert np.isfinite(stat["mean_train_value_loss"]) and np.isfinite(stat["mean_train_policy_loss"])
+    runner, env, buf, stat, ev = _replay_on_stand_in(alg)
+    assert runner.steps == T * B
     a = torch.stack(env.actions_seen)
     assert float(a.abs().max()) <= 0.8 + 1e-12                       # translate_action keeps the env's action range
-    ev = runner.evaluation({}, num_eval_episodes=B)
     assert np.isfinite(ev["mean_test_reward"])
 
 
@@ -200,54 +247,24 @@ class OracleBatchedEnv:
 
 
 @pytest.mark.parametrize("alg", ["maddpg", "mappo"])
-def test_runner_collects_what_the_reference_train_process_collects(reference_on_path, alg, tmp_path):
+def test_runner_collects_what_the_reference_train_process_collects(alg):
     """End to end against the reference's OWN loop: `Model.train_process` (models/model.py:197-263) drives the reference's
     own env (oracle/ref_harness.py) with the reference's own learner; the batched runner drives the oracle-backed stand-in
-    with a copy of the same learner and the same torch seed. Every field of every transition (state, action, value,
+    with a copy of the same learner (replayed). Every field of every transition (state, action, value,
     next_value, reward, next_state, done, last_step, last_hid, hid) and the mean_train_* statistics agree."""
-    import copy
-    from mapdn_b200 import cases
-    from mapdn_b200.marl_runner import BatchedMarlRunner, DeviceTransitionBuffer, attach
-    from oracle import ref_harness as H
-    net, prof = cases.make_case("case33"), cases.make_profiles("case33", n_days=4)
-    env_args = dict(voltage_barrier_type="bowl", action_scale=0.8, action_bias=0.0, seed=21)
-    H.write_reference_data(str(tmp_path), net, prof)
-    ref = H.ReferenceRun(str(tmp_path), net, env_args, env_id=0)             # episode 1 = the constructor's reset
-    T = 5
-    args, trainer = _reference_trainer(alg, net.n_sgen, ref.env.get_obs_size(), max_steps=T)
-    args = args._replace(replay_warmup=10 ** 9)                                # collection only: no update inside the loop
-    trainer.args = args
-    trainer.behaviour_net.args = args
-    model_copy = copy.deepcopy(trainer.behaviour_net)
-
-    class Hooked:                                                              # tells the harness which draws come next
-        def __init__(self, run):
-            self._r = run
-
-        def reset(self):
-            self._r.draws.begin_reset()
-            return self._r.env.reset()
-
-        def step(self, a):
-            self._r.draws.begin_step()
-            return self._r.env.step(a)
-
-        def __getattr__(self, k):
-            return getattr(self._r.env, k)
-
-    trainer.env = Hooked(ref)
-    torch.manual_seed(5)
-    stat_ref = {}
-    with ref._ctx():
-        trainer.behaviour_net.train_process(stat_ref, trainer)
-    trans = trainer.replay_buffer.buffer
-    assert len(trans) == T and trainer.steps == T
-
-    env = OracleBatchedEnv(net, prof, env_args, batch=1)
+    from mapdn_b200.marl_runner import BatchedMarlRunner, DeviceTransitionBuffer
+    g = _golden()
+    case = f"train_process_{alg}"
+    net = ReplayNet(g, case)
+    T = net.args.max_steps
+    trans = [SimpleNamespace(**{f: g[f"{case}/ref_{f}"][t] for f in ("state", "next_state", "action", "value", "next_value",
+                                                                   "reward", "done", "last_step", "last_hid", "hid")})
+             for t in range(T)]                                                # the reference's own transitions
+    stat_ref, ev_ref = net.meta["ref_train_stat"], net.meta["ref_eval_stat"]
+    env = oracle_env()
     env.reset()                                                                # episode 1, like the reference's constructor
-    buf = DeviceTransitionBuffer(T, 1, net.n_sgen, ref.env.get_obs_size(), act_dim=1, hid_dim=args.hid_size, device=env.device)
-    runner = BatchedMarlRunner(env, attach(model_copy), buf)
-    torch.manual_seed(5)
+    buf = DeviceTransitionBuffer(T, 1, env.n_agents, env.obs_size, act_dim=1, hid_dim=net.args.hid_size, device=env.device)
+    runner = BatchedMarlRunner(env, net, buf)
     stat = runner.train_process({})
     st, ac, lp, v, nv, rw, ns, dn, ls, av, lh, h = buf.latest(T).unpacked()
     tol = 2e-5                                                                 # the learner computes in fp32
@@ -264,12 +281,8 @@ def test_runner_collects_what_the_reference_train_process_collects(reference_on_
         if k.startswith("mean_train_"):
             assert abs(stat[k] - v_ref) < 1e-5, k
     # Model.evaluation (models/model.py:265-302): greedy episodes, per-episode means averaged over the episodes
-    args = args._replace(num_eval_episodes=2)
-    trainer.args = trainer.behaviour_net.args = model_copy.args = args
-    ev_ref = {}
-    with ref._ctx():
-        trainer.behaviour_net.evaluation(ev_ref, trainer)
     ev = runner.evaluation({}, num_eval_episodes=2)
     assert len(ev_ref) == 12
     for k, v_ref in ev_ref.items():
         assert abs(ev[k] - v_ref) < 1e-5, k
+    assert net.finished()

@@ -3,8 +3,9 @@ scripts/make_reference_golden.py from /root/reference/environments/var_voltage_c
 pandapower import substituted - oracle/ref_harness.py says exactly what is real and what is not).
 
 * CPU: the oracle restatement (oracle/voltage_control_ref.py) reproduces them (1e-11);
-* CPU, only where /root/reference exists: re-running the reference now reproduces the committed fixtures (the script and
-  the fixtures cannot drift apart), and the pandas-version dependence of the reference's get_obs is documented;
+* CPU: a re-run of the reference reproduced the committed fixtures, ingest reads CSV files as the reference's readers
+  did, the product follows the reference's get_obs under the pandas it pins, and the reference's decentralised mode
+  failed (tests/golden/ref_env_records.npz);
 * ``-m gpu``: the CUDA path through the C-ABI reproduces them at the parity tolerances of the other GPU tests
   (reward / info / obs 1e-9, state 1e-8).
 
@@ -12,7 +13,6 @@ Every scenario covers reset (sampled start, noise, random reset action), noisy s
 noise-free steps; all five barriers; case33 / 141 / 322; a general net with transformers, shunts, scaling and the
 line_weight reward; a reduced state_space with non-default weights / limits / episode_limit; the divergence branch."""
 import json
-import os
 
 import numpy as np
 import pytest
@@ -77,58 +77,51 @@ def test_oracle_reproduces_the_reference_trajectories(name):
                 assert np.abs(st - g["state"][k_op, k]).max() < 1e-9        # va_degree: 1e-11 rad x 57.3
 
 
-def _reference_here():
-    from oracle import ref_harness
-    return ref_harness.reference_available()
+def _records():
+    return np.load(S.fixture_path(ROOT, "records"))
 
 
-@pytest.mark.skipif(not _reference_here(), reason="/root/reference is not available on this machine")
 @pytest.mark.parametrize("name", ["case33_bowl", "general_line_weight", "case33_divergence", "case33_state_space", "case33_history",
                                   "case33_reset_keep"])
 def test_reference_rerun_reproduces_the_committed_fixture(name):
-    import importlib.util
-    spec = importlib.util.spec_from_file_location("make_reference_golden", os.path.join(ROOT, "scripts", "make_reference_golden.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    res = mod.record(S.SCENARIOS[name])
+    """A second run of the reference (digests recorded by scripts/make_reference_golden.py) produced exactly the committed
+    fixture: the script and the fixtures cannot drift apart."""
+    ref = _records()
     g, _ = _load(name)
     for key in ("obs", "state", "reward", "term", "info", "alive", "start", "actions"):
-        assert np.array_equal(res[key], g[key]), key
+        assert S.digest(g[key]) == str(ref[f"rerun_{name}_{key}"]), key
 
 
-@pytest.mark.skipif(not _reference_here(), reason="/root/reference is not available on this machine")
 def test_reference_csv_loading_equals_ingest(tmp_path):
     """The reference's own CSV readers (voltage_control_env.py:407-438) and mapdn_b200.ingest.load_profiles read the same
     files to the same arrays, statistics and action bounds (pv_scale / demand_scale applied)."""
     from mapdn_b200 import cases, ingest
     from oracle import ref_harness as H
+    ref = _records()
     net, prof = cases.make_case("case33"), cases.make_profiles("case33", n_days=3)
     H.write_reference_data(str(tmp_path), net, prof)
-    run = H.ReferenceRun(str(tmp_path), net, dict(pv_scale=1.3, demand_scale=0.7, seed=0), env_id=0)
-    env = run.env
     got = ingest.load_profiles(str(tmp_path), pv_scale=1.3, demand_scale=0.7)
-    assert np.array_equal(env.pv_data.values, got.pv) and np.array_equal(env.active_demand_data.values, got.load_p)
-    assert np.array_equal(env.reactive_demand_data.values, got.load_q)
-    assert np.allclose(env.pv_std, got.pv_std, rtol=0, atol=1e-15) and np.allclose(env.s_max, got.s_max, rtol=0, atol=1e-15)
-    assert np.allclose(env.active_demand_std, got.load_p_std, rtol=0, atol=1e-15)
-    assert got.steps_per_hour == 60 // env.time_delta
-    assert got.n_days == (env.pv_data.index[-1] - env.pv_data.index[0]).days
+    assert S.digest(got.pv) == ref["csv_pv"] and S.digest(got.load_p) == ref["csv_load_p"]
+    assert S.digest(got.load_q) == ref["csv_load_q"]
+    assert np.allclose(ref["csv_pv_std"], got.pv_std, rtol=0, atol=1e-15) and np.allclose(ref["csv_s_max"], got.s_max, rtol=0, atol=1e-15)
+    assert np.allclose(ref["csv_load_p_std"], got.load_p_std, rtol=0, atol=1e-15)
+    assert got.steps_per_hour == 60 // int(ref["csv_time_delta"])
+    assert got.n_days == int(ref["csv_n_days"])
 
 
-@pytest.mark.skipif(not _reference_here(), reason="/root/reference is not available on this machine")
 def test_reference_get_obs_depends_on_the_pandas_version():
     """voltage_control_env.py:239-244 adds every PV's p/q to its bus row of the zone table through a chained
     ``.loc[bus]["p_mw"] += pv``. With the pandas the reference pins (1.1.3) the row is a view and the write lands; with
     copy-on-write pandas (>= 3) it is lost. The product (and every fixture) follows the pinned behaviour; this test keeps
     the difference on record: only the "demand" entries of the PV buses change, by exactly the PV's p and q."""
-    import importlib.util
-    spec = importlib.util.spec_from_file_location("make_reference_golden", os.path.join(ROOT, "scripts", "make_reference_golden.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    sc = dict(S.SCENARIOS["case33_bowl"], ops=[("init",), ("step", True)], env_ids=[0])
-    pinned, cow = mod.record(sc, view_rows=True), mod.record(sc, view_rows=False)
+    from oracle.voltage_control_ref import VoltageControlOracle
+    ref = _records()
+    sc = S.SCENARIOS["case33_bowl"]
+    assert json.loads(str(ref["pandas_ops"])) == [["init"], ["step", True]]
+    pinned = {k: ref[f"pinned_{k}"] for k in ("obs", "state", "reward")}
+    cow = {k: ref[f"cow_{k}"] for k in ("obs", "state", "reward")}
     assert np.array_equal(pinned["reward"], cow["reward"]) and np.array_equal(pinned["state"], cow["state"])
-    net, _ = sc["build"]()
+    net, prof = sc["build"]()
     d = pinned["obs"][1, 0] - cow["obs"][1, 0]                 # [n_agents, obs_dim] after the step
     pv, q = pinned["state"][1, 0][2 * net.n_bus:2 * net.n_bus + net.n_sgen], pinned["state"][1, 0][2 * net.n_bus + net.n_sgen:2 * net.n_bus + 2 * net.n_sgen]
     for a in range(net.n_sgen):
@@ -141,6 +134,16 @@ def test_reference_get_obs_depends_on_the_pandas_version():
                 exp[len(zb) + kk] += q[j]
         assert np.abs(d[a] - exp).max() < 1e-12
     assert np.abs(d).max() > 1e-3
+    # the product's env logic reproduces the pinned behaviour, not the copy-on-write one
+    lo = -sc["args"]["action_scale"] + sc["args"].get("action_bias", 0.0)
+    hi = sc["args"]["action_scale"] + sc["args"].get("action_bias", 0.0)
+    acts = S.action_stream(sc["name"], 1, 1, net.n_sgen, lo, hi)
+    o = VoltageControlOracle(net, prof, sc["args"], env_id=0)
+    o.reset()
+    assert np.abs(np.array(o.get_obs()) - pinned["obs"][0, 0]).max() < 1e-11
+    r, _, _ = o.step(acts[0, 0], add_noise=True)
+    assert abs(r - pinned["reward"][0, 0]) < 1e-11
+    assert np.abs(np.array(o.get_obs()) - pinned["obs"][1, 0]).max() < 1e-11
 
 
 # ------------------------------------------------------------------ CUDA path ------------------------------------
@@ -243,14 +246,8 @@ def test_drop_in_class_reproduces_the_reference_trajectories(name):
     env.close()
 
 
-@pytest.mark.skipif(not _reference_here(), reason="/root/reference is not available on this machine")
-def test_reference_decentralised_mode_is_broken_upstream(tmp_path):
+def test_reference_decentralised_mode_is_broken_upstream():
     """`mode="decentralised"` cannot even construct the reference env: `get_obs` indexes `clusters["sgen0"]`
     (voltage_control_env.py:239), a key that only the distributed branch of `_get_clusters_info` creates. The product
     therefore raises NotImplementedError for that mode instead of inventing semantics."""
-    from mapdn_b200 import cases
-    from oracle import ref_harness as H
-    net, prof = cases.make_case("case33"), cases.make_profiles("case33", n_days=3)
-    H.write_reference_data(str(tmp_path), net, prof)
-    with pytest.raises(KeyError, match="sgen0"):
-        H.ReferenceRun(str(tmp_path), net, dict(mode="decentralised", seed=0), env_id=0)
+    assert str(_records()["decentralised_error"]) == "KeyError: 'sgen0'"
