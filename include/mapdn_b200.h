@@ -237,6 +237,26 @@ mapdn_status mapdn_step_host_f32obs(mapdn_env* env, const double* actions_host, 
                                     double* reward_host, uint8_t* terminated_host, double* info_host,
                                     float* obs_host, void* stream);
 
+/*
+ * Tester records (reference utilities/tester.py:26-55): after manual_reset and after every step the tester reads six
+ * getters. A record row holds them side by side, fp64, in the tester's key order:
+ *   [pv_active n_sgen | pv_reactive n_sgen | bus_active n_bus | bus_reactive n_bus | bus_voltage n_bus | line_loss n_line]
+ * = the values mapdn_get_field returns for P_SGEN, Q_SGEN, P_BUS, Q_BUS, VM, LINE_LOSS at that moment (after a step
+ * pv_active is already the next profile row, as in the reference; a diverged step reports the previous results).
+ * mapdn_record_layout: off[MAPDN_N_RECORD] = start of each of the six blocks, row_len = entries per row.
+ * mapdn_record: one gather launch writing the current row of env b to record_dev + b * record_stride (stride in
+ * doubles, >= row_len) - after a reset.
+ * mapdn_step_record: mapdn_step (same arguments, same outputs) whose kernel also writes every env's row after the step
+ * from the values it already holds - no extra launch. record_dev = NULL is exactly mapdn_step.
+ */
+#define MAPDN_N_RECORD 6
+mapdn_status mapdn_record_layout(const mapdn_env* env, int32_t* off /*[MAPDN_N_RECORD]*/, int32_t* row_len);
+mapdn_status mapdn_record(mapdn_env* env, double* record_dev, int64_t record_stride, void* stream);
+mapdn_status mapdn_step_record(mapdn_env* env, const double* actions_dev /*[B,n_sgen]*/, int32_t add_noise,
+                               double* reward_dev /*[B]*/, uint8_t* terminated_dev /*[B]*/,
+                               double* info_dev /*[B,11] or NULL*/, double* obs_dev /*or NULL*/,
+                               double* record_dev /*or NULL*/, int64_t record_stride, void* stream);
+
 mapdn_status mapdn_get_obs(mapdn_env* env, double* obs_dev, void* stream);      /* :232-316 */
 mapdn_status mapdn_get_state(mapdn_env* env, double* state_dev, void* stream);  /* :213-230 */
 mapdn_status mapdn_get_field(mapdn_env* env, int32_t field, double* out_dev, void* stream);

@@ -68,7 +68,10 @@ class DimsC(C.Structure):
 
 EXPORTS = ("mapdn_abi_version", "mapdn_last_error", "mapdn_create", "mapdn_destroy", "mapdn_get_dims",
            "mapdn_reset", "mapdn_step", "mapdn_step_host", "mapdn_step_f32obs", "mapdn_step_host_f32obs", "mapdn_step_host_pinned", "mapdn_wait", "mapdn_obs_compact_layout", "mapdn_step_host_compact", "mapdn_get_obs", "mapdn_get_state",
-           "mapdn_get_field", "mapdn_solve", "mapdn_droop", "mapdn_get_ybus_dense", "mapdn_launch_count")
+           "mapdn_get_field", "mapdn_solve", "mapdn_droop", "mapdn_get_ybus_dense", "mapdn_launch_count",
+           "mapdn_record_layout", "mapdn_record", "mapdn_step_record")
+# tester record row blocks, in the reference tester's key order (utilities/tester.py:26-32); mapdn_record_layout
+RECORD_KEYS = ("pv_active", "pv_reactive", "bus_active", "bus_reactive", "bus_voltage", "line_loss")
 
 _lib: Optional[C.CDLL] = None
 
@@ -105,6 +108,9 @@ def lib() -> C.CDLL:
         L.mapdn_droop.argtypes = [vp, C.c_int32] + [vp] * 5 + [C.c_double, C.c_double, C.c_int32] + [vp] * 5
         L.mapdn_obs_compact_layout.argtypes = [vp, vp, vp, vp]
         L.mapdn_step_host_compact.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp]
+        L.mapdn_record_layout.argtypes = [vp, vp, vp]
+        L.mapdn_record.argtypes = [vp, vp, C.c_int64, vp]
+        L.mapdn_step_record.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, vp, C.c_int64, vp]
     except AttributeError:
         if not dev_override:
             raise

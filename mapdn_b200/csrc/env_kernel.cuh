@@ -757,9 +757,12 @@ __device__ __forceinline__ double clip_q(double a, double pv, double smax) {
   return sqrt(smax * smax - pv * pv) * a;
 }
 
-template <int G, int MODE, bool DENSE = false>
+// RECORD (MODE_STEP only): the epilogue also writes the env's tester record row (see Params::record) from the values it
+// already holds. A template flag, so the instantiations without it are the same code as before it existed.
+template <int G, int MODE, bool DENSE = false, bool RECORD = false>
 __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_constant__ Params p) {
   static_assert(!DENSE || G == 32, "the dense fallback uses one warp per env");
+  static_assert(!RECORD || MODE == MODE_STEP, "records are written by the step kernel");
   static_assert(G == 4 || G == 8 || G == 16 || G == 32 || G == 64 || G == 128, "unsupported group size");
 #ifdef MAPDN_HOST_EMU
   unsigned char* const smem_raw = emu::dyn_smem();
@@ -1141,9 +1144,17 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
     }
     // the helper warp has drawn the next profile row meanwhile: take over the new sgen.p_mw (Appendix B.3: the
     // observation mixes this solve's bus results with the NEXT row's PV)
+    // record row [pv | q | P_bus | Q_bus | vm | line loss] (the order of the reference tester's getters): exactly what
+    // mapdn_get_field returns after this step. pv is already the next profile row (reference :199 runs before the
+    // tester's getters); q is the effective one; a diverged env reports its previous results, read back from HBM.
+    double* const rec = RECORD ? p.record + static_cast<size_t>(env) * p.record_stride : nullptr;
     if (MODE == MODE_STEP) {
       named_bar_sync(2, blockDim.x);
       for (int j = gl; j < ng; j += G) s.pv[j] = next_row[j];
+      if constexpr (RECORD) {
+        if (valid)
+          for (int j = gl; j < ng; j += G) { rec[j] = s.pv[j]; rec[ng + j] = s.q[j]; }
+      }
     }
     grp_sync<G>(gidx);
     PROF(8)
@@ -1182,6 +1193,13 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
         if (write_res) {
           p.res_vm[eN + b] = v; p.res_va[eN + b] = th; p.res_p[eN + b] = bp.x; p.res_q[eN + b] = bp.y;
         }
+        if constexpr (RECORD) {         // consecutive lanes, consecutive buses: coalesced like the res_* stores
+          if (valid) {
+            rec[2 * ng + b] = conv ? bp.x : p.res_p[eN + b];
+            rec[2 * ng + n + b] = conv ? bp.y : p.res_q[eN + b];
+            rec[2 * ng + 2 * n + b] = v;                    // on divergence: reloaded from res_vm above
+          }
+        }
         if (MODE == MODE_STEP) {
           cnt_lo += (v < p.v_lower) ? 1.0 : 0.0;
           cnt_hi += (v > p.v_upper) ? 1.0 : 0.0;
@@ -1209,6 +1227,9 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
           sum_pl += pl;
           if (kExplicit) { if (valid && p.out_pl) p.out_pl[ePL + k] = pl; }
           else if (write_res) p.res_pl[ePL + k] = pl;
+          if constexpr (RECORD) {
+            if (valid) rec[2 * ng + 3 * n + k] = conv ? pl : p.res_pl[ePL + k];
+          }
         }
       };
       if (h.in_blob) lines(reinterpret_cast<const ushort2*>(smem_raw + hl.line_nodes), reinterpret_cast<const double2*>(smem_raw + hl.line_c));

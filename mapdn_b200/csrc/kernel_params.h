@@ -131,6 +131,10 @@ struct Params {
   double* dense_ws;       // meshed nets only: per resident env group, (2 npq) x (2 npq + 1) doubles [J | rhs]
   int dense_stride;       // doubles per group in dense_ws
   long long* prof;        // MAPDN_PROFILE builds: per-phase clock64 totals of warp 0 of block 0
+  // tester records (mapdn_step_record / mapdn_record): row of env b at record + b * record_stride (doubles), laid out
+  // [pv n_sgen | q n_sgen | P_bus n_bus | Q_bus n_bus | vm n_bus | line loss n_line]
+  double* record;
+  long long record_stride;
 };
 
 // cold obs program entry: kind in the top 4 bits, node / sgen index in the low 28

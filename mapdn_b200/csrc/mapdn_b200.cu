@@ -157,6 +157,23 @@ __global__ void get_state_kernel(const __grid_constant__ Params p) {
   p.state[gid] = v;
 }
 
+// mapdn_record: the tester record row of every env from the state in HBM (the six get_field columns side by side)
+__global__ void record_kernel(const __grid_constant__ Params p) {
+  const int ng = p.n_sgen, n = p.n_bus, row = 2 * ng + 3 * n + p.n_line;
+  const long long gid = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  if (gid >= static_cast<long long>(p.nb) * row) return;
+  const int env = static_cast<int>(gid / row), k = static_cast<int>(gid - static_cast<long long>(env) * row);
+  const size_t eN = static_cast<size_t>(env) * n, eG = static_cast<size_t>(env) * ng;
+  double v;
+  if (k < ng) v = p.cur_pv[eG + k];
+  else if (k < 2 * ng) v = p.cur_q[eG + k - ng];
+  else if (k < 2 * ng + n) v = p.res_p[eN + k - 2 * ng];
+  else if (k < 2 * ng + 2 * n) v = p.res_q[eN + k - 2 * ng - n];
+  else if (k < 2 * ng + 3 * n) v = p.res_vm[eN + k - 2 * ng - 2 * n];
+  else v = p.res_pl[static_cast<size_t>(env) * p.n_line + k - 2 * ng - 3 * n];
+  p.record[static_cast<size_t>(env) * p.record_stride + k] = v;
+}
+
 }  // namespace mapdn
 
 using namespace mapdn;
@@ -169,6 +186,7 @@ struct mapdn_env {
   Params base{};                       // static + state pointers; io fields filled per call
   std::vector<void*> allocs;           // everything cudaMalloc'ed
   int G = 8, threads = 128, epb = 16, smem = 0, max_blocks = 0, helper_threads = 32;
+  int max_blocks_record = 0;           // persistent grid of the MODE_STEP instantiation with tester records
   bool dense = false;                  // meshed net: dense-LU fallback solver
   long long launches = 0;
   // Ybus pieces kept for the test hook
@@ -216,31 +234,32 @@ using KernelFn = void (*)(const Params);
 constexpr int kHelperPairsPerWarp = 256;   // Box-Muller pairs of a CTA round per helper warp
 
 template <int G>
-KernelFn kernel_for_mode(int mode) {
+KernelFn kernel_for_mode(int mode, bool record) {
   switch (mode) {
     case MODE_SOLVE: return env_kernel<G, MODE_SOLVE>;
-    case MODE_STEP: return env_kernel<G, MODE_STEP>;
+    case MODE_STEP: return record ? env_kernel<G, MODE_STEP, false, true> : env_kernel<G, MODE_STEP>;
     case MODE_DROOP: return env_kernel<G, MODE_DROOP>;
     default: return env_kernel<G, MODE_RESET>;
   }
 }
 
-KernelFn kernel_for(int G, int mode, bool dense = false) {
+// record: the MODE_STEP instantiation that also writes the tester record rows (mapdn_step_record)
+KernelFn kernel_for(int G, int mode, bool dense = false, bool record = false) {
   if (dense) {
     switch (mode) {
       case MODE_SOLVE: return env_kernel<32, MODE_SOLVE, true>;
-      case MODE_STEP: return env_kernel<32, MODE_STEP, true>;
+      case MODE_STEP: return record ? env_kernel<32, MODE_STEP, true, true> : env_kernel<32, MODE_STEP, true>;
       case MODE_DROOP: return env_kernel<32, MODE_DROOP, true>;
       default: return env_kernel<32, MODE_RESET, true>;
     }
   }
   switch (G) {
-    case 4: return kernel_for_mode<4>(mode);
-    case 8: return kernel_for_mode<8>(mode);
-    case 16: return kernel_for_mode<16>(mode);
-    case 64: return kernel_for_mode<64>(mode);
-    case 128: return kernel_for_mode<128>(mode);
-    default: return kernel_for_mode<32>(mode);
+    case 4: return kernel_for_mode<4>(mode, record);
+    case 8: return kernel_for_mode<8>(mode, record);
+    case 16: return kernel_for_mode<16>(mode, record);
+    case 64: return kernel_for_mode<64>(mode, record);
+    case 128: return kernel_for_mode<128>(mode, record);
+    default: return kernel_for_mode<32>(mode, record);
   }
 }
 
@@ -264,9 +283,10 @@ int env_stride2_for(int npq, int ng, int nl, int G, bool stage_rec) {
 }
 
 mapdn_status launch_env_kernel(mapdn_env* e, int mode, Params& p, cudaStream_t st) {
-  KernelFn fn = kernel_for(e->G, mode, e->dense);
+  const bool record = mode == MODE_STEP && p.record != nullptr;
+  KernelFn fn = kernel_for(e->G, mode, e->dense, record);
   const int needed = (p.nb + e->epb - 1) / e->epb;
-  int grid = std::min(needed, std::max(1, e->max_blocks));
+  int grid = std::min(needed, std::max(1, record ? e->max_blocks_record : e->max_blocks));
   const int rounds = (needed + grid - 1) / grid;
   grid = (needed + rounds - 1) / rounds;       // balance the persistent loop
 #ifdef MAPDN_PROFILE
@@ -995,8 +1015,8 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
     e->helper_threads = 32 * std::min(4, std::max(1, (epb * n_pair + kHelperPairsPerWarp - 1) / kHelperPairsPerWarp));
   }
   if (const char* ov = getenv("MAPDN_HELPERS")) e->helper_threads = 32 * std::min(4, std::max(1, atoi(ov)));   // tuning override
-  for (int mode = 0; mode < 4; ++mode) {
-    KernelFn fn = kernel_for(G, mode, meshed);
+  for (int mode = 0; mode < 5; ++mode) {      // 4: the MODE_STEP instantiation with tester records
+    KernelFn fn = (mode < 4) ? kernel_for(G, mode, meshed) : kernel_for(G, MODE_STEP, meshed, true);
     // the attribute belongs to the function, not to the handle: always allow the device maximum, so that creating a
     // second handle with a smaller footprint cannot break the launches of the first
     cudaFuncAttributes fa{};
@@ -1011,6 +1031,9 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
     TRY_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel_for(G, MODE_STEP, meshed), e->threads + e->helper_threads, e->smem));
     e->max_blocks = std::max(1, per_sm) * dp.multiProcessorCount;
     if (meshed) e->max_blocks = std::min(e->max_blocks, 2 * dp.multiProcessorCount);   // bounds the dense workspace
+    // the record instantiation holds more registers: its persistent grid is sized by its own occupancy (never larger)
+    TRY_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel_for(G, MODE_STEP, meshed, true), e->threads + e->helper_threads, e->smem));
+    e->max_blocks_record = std::min(e->max_blocks, std::max(1, per_sm) * dp.multiProcessorCount);
   }
 
   // ---- 6. upload + env state ----
@@ -1212,6 +1235,44 @@ mapdn_status mapdn_step(mapdn_env* e, const double* actions_dev, int32_t add_noi
   Params p = e->base;
   p.actions = actions_dev; p.add_noise = add_noise; p.reward = reward_dev; p.term = terminated_dev;
   p.info = info_dev; p.obs = obs_dev;
+  return launch_env_kernel(e, MODE_STEP, p, static_cast<cudaStream_t>(stream));
+}
+
+static int record_row_len(const mapdn_env* e) { return 2 * e->dims.n_sgen + 3 * e->dims.n_bus + e->dims.n_line; }
+
+mapdn_status mapdn_record_layout(const mapdn_env* e, int32_t* off, int32_t* row_len) {
+  if (!e) return fail(MAPDN_ERR_INVALID, "null handle");
+  const int ng = e->dims.n_sgen, n = e->dims.n_bus;
+  const int32_t o[MAPDN_N_RECORD] = {0, ng, 2 * ng, 2 * ng + n, 2 * ng + 2 * n, 2 * ng + 3 * n};
+  if (off) for (int k = 0; k < MAPDN_N_RECORD; ++k) off[k] = o[k];
+  if (row_len) *row_len = record_row_len(e);
+  return MAPDN_OK;
+}
+
+mapdn_status mapdn_record(mapdn_env* e, double* record_dev, int64_t record_stride, void* stream) {
+  if (!e || !record_dev) return fail(MAPDN_ERR_INVALID, "null argument");
+  if (record_stride < record_row_len(e)) return fail(MAPDN_ERR_INVALID, "record_stride shorter than a record row");
+  MAPDN_ON_DEVICE(e->device);
+  Params p = e->base;
+  p.record = record_dev; p.record_stride = record_stride;
+  const long long tot = static_cast<long long>(p.nb) * record_row_len(e);
+  MAPDN_LAUNCH(record_kernel, static_cast<unsigned>((tot + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream), p);
+  MAPDN_CUDA(cudaGetLastError());
+  e->launches++;
+  return MAPDN_OK;
+}
+
+mapdn_status mapdn_step_record(mapdn_env* e, const double* actions_dev, int32_t add_noise, double* reward_dev,
+                               uint8_t* terminated_dev, double* info_dev, double* obs_dev, double* record_dev,
+                               int64_t record_stride, void* stream) {
+  if (!e || !actions_dev || !reward_dev || !terminated_dev) return fail(MAPDN_ERR_INVALID, "null argument");
+  if (!e->base.prof_pv) return fail(MAPDN_ERR_INVALID, "handle was created without a profile store");
+  if (record_dev && record_stride < record_row_len(e)) return fail(MAPDN_ERR_INVALID, "record_stride shorter than a record row");
+  MAPDN_ON_DEVICE(e->device);
+  Params p = e->base;
+  p.actions = actions_dev; p.add_noise = add_noise; p.reward = reward_dev; p.term = terminated_dev;
+  p.info = info_dev; p.obs = obs_dev;
+  p.record = record_dev; p.record_stride = record_stride;
   return launch_env_kernel(e, MODE_STEP, p, static_cast<cudaStream_t>(stream));
 }
 

@@ -192,15 +192,25 @@ class BatchedVoltageControl:
             self._hist[:, -1] = self.obs
         return self.obs, self.state
 
-    def step(self, actions: torch.Tensor, add_noise: bool = True, want_obs: bool = True, want_info: bool = True):
+    def step(self, actions: torch.Tensor, add_noise: bool = True, want_obs: bool = True, want_info: bool = True,
+             record: Optional[torch.Tensor] = None):
         """One transition of every env. Returns (reward ``[B]``, terminated ``[B]`` uint8,
-        info ``[B,11]`` in INFO_KEYS order); the new observations are in ``self.obs``."""
+        info ``[B,11]`` in INFO_KEYS order); the new observations are in ``self.obs``.
+
+        ``record``: an fp64 ``[B, record_len]`` view with unit column stride and any row stride (row ``t`` of a
+        ``[B, T + 1, record_len]`` tensor): the same kernel launch also writes every env's tester record after the step
+        (:attr:`record_slices`, ``mapdn_step_record``)."""
         if (actions.dtype is not torch.float64 or tuple(actions.shape) != self._act_shape or actions.device != self.device
                 or not actions.is_contiguous()):
             self._chk(actions, self._act_shape, name="actions")
-        st = self._L.mapdn_step(self._h, actions.data_ptr(), int(add_noise), self._p_reward, self._p_term,
-                                self._p_info if want_info else None, self._p_obs if want_obs else None,
-                                torch.cuda.current_stream(self.device).cuda_stream)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        if record is not None:
+            st = self._L.mapdn_step_record(self._h, actions.data_ptr(), int(add_noise), self._p_reward, self._p_term,
+                                           self._p_info if want_info else None, self._p_obs if want_obs else None,
+                                           record.data_ptr(), self._record_stride(record), stream)
+        else:
+            st = self._L.mapdn_step(self._h, actions.data_ptr(), int(add_noise), self._p_reward, self._p_term,
+                                    self._p_info if want_info else None, self._p_obs if want_obs else None, stream)
         if st:
             _capi.check(st)
         if self.history > 1 and want_obs and self._hist is not None:
@@ -332,6 +342,38 @@ class BatchedVoltageControl:
                      sum_rewards=1, steps=1, start_row=1, nr_iters=1)[name]
         out = torch.empty(self.batch, width, dtype=torch.float64, device=self.device)
         _capi.check(self._L.mapdn_get_field(self._h, _capi.FIELDS[name], _ptr(out), self._stream()))
+        return out
+
+    # ---- tester records (reference utilities/tester.py:26-55) ---------------------------------------
+    @property
+    def record_slices(self):
+        """``{key: (offset, length)}`` of the six blocks of a tester record row, in the reference tester's key order
+        (``RECORD_KEYS``: pv_active, pv_reactive, bus_active, bus_reactive, bus_voltage, line_loss)."""
+        if getattr(self, "_record_slices", None) is None:
+            off, row = (C.c_int32 * len(_capi.RECORD_KEYS))(), C.c_int32(0)
+            _capi.check(self._L.mapdn_record_layout(self._h, off, C.byref(row)))
+            ends = [int(o) for o in off][1:] + [int(row.value)]
+            self._record_slices = {k: (int(o), e - int(o)) for k, o, e in zip(_capi.RECORD_KEYS, off, ends)}
+            self._record_len = int(row.value)
+        return self._record_slices
+
+    @property
+    def record_len(self) -> int:
+        """Entries of one tester record row."""
+        self.record_slices
+        return self._record_len
+
+    def _record_stride(self, out: torch.Tensor) -> int:
+        if (out.dtype is not torch.float64 or out.device != self.device or out.dim() != 2
+                or tuple(out.shape) != (self.batch, self.record_len) or out.stride(1) != 1):
+            raise ValueError(f"record: expected a float64 [{self.batch}, {self.record_len}] view with unit column stride on "
+                             f"{self.device}, got {out.dtype} {tuple(out.shape)} strides {out.stride()} on {out.device}")
+        return out.stride(0)
+
+    def record(self, out: torch.Tensor) -> torch.Tensor:
+        """The current tester record row of every env into ``out`` (``[B, record_len]`` view, any row stride): one gather
+        launch. After a step, :meth:`step` with ``record=`` writes the same rows without it."""
+        _capi.check(self._L.mapdn_record(self._h, out.data_ptr(), self._record_stride(out), self._stream()))
         return out
 
     def get_avail_actions(self) -> torch.Tensor:

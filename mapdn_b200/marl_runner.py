@@ -30,7 +30,8 @@ import torch
 from ._capi import INFO_KEYS
 from .rollout import translate_action
 
-__all__ = ["TRANSITION_FIELDS", "DeviceBatch", "DeviceTransitionBuffer", "attach", "BatchedMarlRunner"]
+__all__ = ["TRANSITION_FIELDS", "DeviceBatch", "DeviceTransitionBuffer", "attach", "BatchedMarlRunner",
+           "BatchedPolicyTester"]
 
 # reference models/model.py:18
 TRANSITION_FIELDS = ("state", "action", "log_prob_a", "value", "next_value", "reward", "next_state", "done",
@@ -236,3 +237,107 @@ class BatchedMarlRunner:
         for k, v in zip(INFO_KEYS, tot[1:]):
             stat["mean_test_" + k] = v
         return stat
+
+
+class BatchedPolicyTester:
+    """The reference's ``PGTester`` (``utilities/tester.py``) over B lock-step envs: ``run`` becomes :meth:`test_run`
+    (one env per test day, the six tester getters written by the step kernel itself) and ``batch_run`` becomes
+    :meth:`test_batch_run` (B episodes at a time, statistics pooled on the device). Same model interface as
+    :class:`BatchedMarlRunner`, whose hidden-state and ``translate_action`` helpers it uses. Needs an env with the record
+    surface of ``BatchedVoltageControl`` (``record_slices``, ``record_len``, ``record(out)``, ``step(..., record=)``)."""
+
+    def __init__(self, env, net):
+        self.env, self.net, self.args = env, net, net.args
+        self._runner = BatchedMarlRunner(env, net)
+        self.records, self.lengths = None, None
+
+    def _act(self, state, last_hid):
+        action, _, _, _, hid = self.net.get_actions(state, status="test", exploration=False, actions_avail=self._runner._avail,
+                                                    target=False, last_hid=last_hid)
+        return self._runner._translate(action), hid
+
+    @torch.no_grad()
+    def test_run(self, days, hour: int = 23, interval: int = 2):
+        """``PGTester.run(day, hour, interval)`` for every day of ``days`` (tester.py:19-63): ``manual_reset`` (noise-free
+        start, reset action drawn as in the reference), then noise-free steps of the policy with its hidden state
+        carried, until ``done or t == max_steps - 1``. Returns ``records [n_days, max_steps + 1, record_len]`` (fp64, on
+        the env's device; rows past an env's end are NaN) and ``lengths [n_days]`` (rows of each day's record). More days
+        than the env's batch run in chunks of B. :meth:`records_for_day` gives one day in the reference's structure."""
+        env, T = self.env, int(self.args.max_steps)
+        days = [int(d) for d in days]
+        B, R, dev = env.batch, env.record_len, env.device
+        nan = float("nan")
+        records = torch.full((len(days), T + 1, R), nan, dtype=torch.float64, device=dev)
+        lengths = torch.zeros(len(days), dtype=torch.int64, device=dev)
+        for c0 in range(0, len(days), B):
+            chunk = days[c0:c0 + B]
+            n = len(chunk)
+            # a short last chunk repeats its first day in the spare envs (their rows are dropped)
+            start = torch.tensor([[d, hour, interval] for d in chunk + chunk[:1] * (B - n)], dtype=torch.int32, device=dev)
+            buf = records[c0:c0 + n] if n == B else torch.full((B, T + 1, R), nan, dtype=torch.float64, device=dev)
+            env.reset(start, add_noise=False, check=True)                                     # tester.py:21
+            env.record(buf[:, 0])                                                             # :34-39
+            state = env.obs.to(torch.float32).clone()
+            last_hid = self._runner._init_hidden()
+            alive = torch.ones(B, dtype=torch.bool, device=dev)
+            length = torch.ones(B, dtype=torch.int64, device=dev)
+            for t in range(T):
+                actions, hid = self._act(state, last_hid)
+                _, done, _ = env.step(actions, add_noise=False, record=buf[:, t + 1])           # :48-55
+                length += alive
+                alive &= done == 0                                                            # :49, :61
+                state, last_hid = env.obs.to(torch.float32).clone(), hid
+            rows = torch.arange(T + 1, device=dev)[None, :, None]
+            buf.masked_fill_(rows >= length[:, None, None], nan)
+            if n < B:
+                records[c0:c0 + n] = buf[:n]
+            lengths[c0:c0 + n] = length[:n]
+        self.records, self.lengths = records, lengths
+        return records, lengths
+
+    def records_for_day(self, i: int) -> dict:
+        """Day ``i`` of the last :meth:`test_run` as ``PGTester.run`` returns it: a dict of six lists of 1-D arrays (one
+        per reset / step), keys in the tester's order - pickling it gives the file ``test.py`` writes."""
+        n = int(self.lengths[i])
+        rows = self.records[i, :n].cpu().numpy()
+        return {k: [rows[t, o:o + w].copy() for t in range(n)] for k, (o, w) in self.env.record_slices.items()}
+
+    @torch.no_grad()
+    def test_batch_run(self, num_episodes: int = 100) -> dict:
+        """``PGTester.batch_run(num_episodes)`` (tester.py:65-99): sampled resets with noise (as ``reset()``), noise-free
+        steps, every info key pooled over every step of every episode up to its ``done_``, reported as
+        ``{"mean_test_<key>": (mean, 2 * std)}`` (``np.mean`` / population ``np.std``). Episode ``e`` runs on env
+        ``e % B`` in round ``e // B``; the statistics are combined on the device, one host read at the end."""
+        env, T = self.env, int(self.args.max_steps)
+        B, dev, K = env.batch, env.device, len(INFO_KEYS)
+        num_episodes = int(num_episodes)
+        n = torch.zeros((), dtype=torch.float64, device=dev)
+        mean = torch.zeros(K, dtype=torch.float64, device=dev)
+        m2 = torch.zeros(K, dtype=torch.float64, device=dev)
+        vals = torch.zeros(T, B, K, dtype=torch.float64, device=dev)
+        mask = torch.zeros(T, B, dtype=torch.float64, device=dev)
+        for r0 in range(0, num_episodes, B):
+            vals.zero_(); mask.zero_()
+            env.reset(check=True)                                                             # tester.py:69
+            state = env.obs.to(torch.float32).clone()
+            last_hid = self._runner._init_hidden()
+            alive = torch.arange(B, device=dev) < num_episodes - r0                           # spare envs of the last round
+            for t in range(T):
+                actions, hid = self._act(state, last_hid)
+                _, done, info = env.step(actions, add_noise=False)                            # :81
+                vals[t] = info
+                mask[t] = alive.to(torch.float64)                                             # :84-88
+                alive &= done == 0                                                            # :82, :93
+                state, last_hid = env.obs.to(torch.float32).clone(), hid
+            # this round's pooled statistics (two-pass), merged into the running ones (Chan et al.)
+            nr = mask.sum()
+            mr = (vals * mask[..., None]).sum(dim=(0, 1)) / nr
+            m2r = (((vals - mr) ** 2) * mask[..., None]).sum(dim=(0, 1))
+            tot = n + nr
+            delta = mr - mean
+            mean = mean + delta * (nr / tot)
+            m2 = m2 + m2r + delta ** 2 * (n * nr / tot)
+            n = tot
+        std = torch.sqrt(m2 / n)
+        out = torch.stack([mean, 2.0 * std], dim=1).tolist()                                # the one host read
+        return {"mean_test_" + k: (v[0], v[1]) for k, v in zip(INFO_KEYS, out)}
