@@ -984,7 +984,8 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
       if (fits(c)) { c_epb = std::max(c_epb, c); break; }
     }
     if (const char* ov = getenv("MAPDN_EPB")) c_epb = std::max(unit, atoi(ov) / unit * unit);   // tuning override
-    while (c_epb > unit && (smem_with(cold, pl.st2, c_epb) > max_smem || (G <= 32 && c_epb * G > 256))) c_epb -= unit;
+    // the override obeys the search's caps too: 256 / 512 solver threads (launch bounds, named-barrier ids 3 + gidx <= 15)
+    while (c_epb > unit && (smem_with(cold, pl.st2, c_epb) > max_smem || c_epb * G > (G <= 32 ? 256 : 512))) c_epb -= unit;
     pl.epb = c_epb;
     pl.ok = smem_with(cold, pl.st2, c_epb) <= max_smem;
     pl.rounds = (cfg->batch + static_cast<long long>(c_epb) * n_sm - 1) / (static_cast<long long>(c_epb) * n_sm);

@@ -79,9 +79,12 @@ static inline cudaError_t cudaMemsetAsync(void* d, int v, size_t n, cudaStream_t
 static inline cudaError_t cudaPointerGetAttributes(cudaPointerAttributes* a, const void* p) {   // every host buffer counts as pinned
   a->type = cudaMemoryTypeHost; a->device = 0; a->devicePointer = const_cast<void*>(p); a->hostPointer = const_cast<void*>(p); return cudaSuccess;
 }
-static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp* p, int) {                      // the H100 SXM numbers the host code plans with
+// the H100 SXM numbers the host code plans with; MAPDN_EMU_SMS=<n> shrinks the SM count, so that a handful of envs gets the
+// launch geometry (envs per CTA, shared-memory plan, persistent rounds) of a benchmark-size batch
+static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp* p, int) {
   memset(p, 0, sizeof(*p)); snprintf(p->name, sizeof(p->name), "emulated H100");
-  p->multiProcessorCount = 132; p->sharedMemPerBlockOptin = 232448; p->sharedMemPerMultiprocessor = 233472; p->reservedSharedMemPerBlock = 1024;
+  const char* sms = getenv("MAPDN_EMU_SMS");
+  p->multiProcessorCount = (sms && atoi(sms) > 0) ? atoi(sms) : 132; p->sharedMemPerBlockOptin = 232448; p->sharedMemPerMultiprocessor = 233472; p->reservedSharedMemPerBlock = 1024;
   p->major = 9; p->minor = 0; p->totalGlobalMem = size_t(80) << 30; p->maxThreadsPerMultiProcessor = 2048; p->regsPerMultiprocessor = 65536;
   p->sharedMemPerBlock = 49152; p->warpSize = 32; return cudaSuccess;
 }
@@ -138,11 +141,15 @@ struct emu_uint3 { unsigned x, y, z; };
 extern thread_local emu_uint3 threadIdx, blockIdx;
 extern thread_local dim3 blockDim, gridDim;
 
+namespace emu { extern std::atomic<unsigned> g_last_grid; }   // CTAs of the last launch: the tests derive the rounds from it
+
 #ifdef MAPDN_EMU_DEFINE_GLOBALS
 thread_local emu::ThreadCtx emu::tctx;
 std::atomic<long long> emu::g_deadline_ms{0};
+std::atomic<unsigned> emu::g_last_grid{0};
 thread_local emu_uint3 threadIdx, blockIdx;
 thread_local dim3 blockDim, gridDim;
+extern "C" __attribute__((visibility("default"))) int mapdn_emu_last_grid() { return int(emu::g_last_grid.load()); }
 #endif
 
 namespace emu {
@@ -152,6 +159,7 @@ inline unsigned char* dyn_smem() { return tctx.blk->smem; }
 template <class F> void launch_impl(unsigned grid, unsigned block, size_t smem_bytes, F&& body) {
   const char* to = getenv("MAPDN_EMU_TIMEOUT_S");
   const long long budget_ms = 1000ll * (to ? atoll(to) : 120);
+  g_last_grid.store(grid);
   for (unsigned b = 0; b < grid; ++b) {
     Block blk;
     blk.nthreads = int(block);

@@ -117,11 +117,17 @@ class EmuEnv:
                                     ("vm", "va_deg", "p_bus", "q_bus", "pl", "iterations", "converged")], None))
         return out
 
-    def reset(self, start=None, add_noise=True):
+    def reset(self, start=None, add_noise=True, mask=None):
         st = None if start is None else np.ascontiguousarray(start, np.int32)
-        self._chk(lib().mapdn_reset(self._h, _ptr(st), None, int(add_noise), _ptr(self.obs), _ptr(self.state),
+        mk = None if mask is None else np.ascontiguousarray(mask, np.uint8)
+        self._chk(lib().mapdn_reset(self._h, _ptr(st), _ptr(mk), int(add_noise), _ptr(self.obs), _ptr(self.state),
                                     _ptr(self.reset_ok), None))
         return self.obs, self.state
+
+    @staticmethod
+    def last_grid():
+        """CTAs of the last emulated kernel launch (the persistent loop runs ceil(ceil(B / epb) / grid) rounds)."""
+        return int(lib().mapdn_emu_last_grid())
 
     def step(self, actions, add_noise=True):
         a = np.ascontiguousarray(actions, np.float64)
