@@ -25,12 +25,14 @@ INFO_KEYS = ("percentage_of_v_out_of_control", "percentage_of_lower_than_lower_v
              "max_voltage_rise_deviation", "total_line_loss", "q_loss", "destroy")
 FIELDS = dict(vm=0, va_deg=1, p_bus=2, q_bus=3, p_sgen=4, q_sgen=5, line_loss=6, p_load=7, q_load=8,
               sum_rewards=9, steps=10, start_row=11, nr_iters=12)
+# get_field columns per env: the dims entry named here; the fields not named have one
+FIELD_DIMS = dict(vm="n_bus", va_deg="n_bus", p_bus="n_bus", q_bus="n_bus", p_sgen="n_sgen", q_sgen="n_sgen",
+                  line_loss="n_line", p_load="n_load", q_load="n_load")
 
 ABI_VERSION = 2
 
-_pd = C.POINTER(C.c_double)
-_pi = C.POINTER(C.c_int32)
-_pb = C.POINTER(C.c_uint8)
+_pd, _pi, _pb = C.POINTER(C.c_double), C.POINTER(C.c_int32), C.POINTER(C.c_uint8)
+_vp, _i32, _i64 = C.c_void_p, C.c_int32, C.c_int64
 
 
 class NetDescC(C.Structure):
@@ -66,10 +68,22 @@ class DimsC(C.Structure):
         ("algorithmic_bytes_per_env_step", C.c_int64)]
 
 
-EXPORTS = ("mapdn_abi_version", "mapdn_last_error", "mapdn_create", "mapdn_destroy", "mapdn_get_dims",
-           "mapdn_reset", "mapdn_step", "mapdn_step_host", "mapdn_step_f32obs", "mapdn_step_host_f32obs", "mapdn_step_host_pinned", "mapdn_wait", "mapdn_obs_compact_layout", "mapdn_step_host_compact", "mapdn_get_obs", "mapdn_get_state",
-           "mapdn_get_field", "mapdn_solve", "mapdn_droop", "mapdn_get_ybus_dense", "mapdn_launch_count",
-           "mapdn_record_layout", "mapdn_record", "mapdn_step_record")
+_STEP = [_vp, _vp, _i32] + [_vp] * 5                             # handle, actions, add_noise, four outputs, stream
+_STEP_HOST = _STEP[:-1] + [_i32] * 3 + [_vp]                     # obs_is_f32 and two flags before the stream
+# every entry point of include/mapdn_b200.h: name -> (argtypes, restype); a mapdn_status is an int32
+SIGNATURES = dict(
+    mapdn_abi_version=([], _i32), mapdn_last_error=([], C.c_char_p), mapdn_launch_count=([_vp], _i64),
+    mapdn_create=([C.POINTER(NetDescC), C.POINTER(ProfileDescC), C.POINTER(CfgC), _i32, C.POINTER(_vp)], _i32),
+    mapdn_destroy=([_vp], _i32), mapdn_get_dims=([_vp, C.POINTER(DimsC)], _i32), mapdn_wait=([_vp] * 2, _i32),
+    mapdn_reset=([_vp, _vp, _vp, _i32] + [_vp] * 4, _i32), mapdn_step=(_STEP, _i32), mapdn_step_f32obs=(_STEP, _i32),
+    mapdn_step_host=(_STEP, _i32), mapdn_step_host_f32obs=(_STEP, _i32), mapdn_step_host_pinned=(_STEP_HOST, _i32),
+    mapdn_step_host_compact=(_STEP_HOST, _i32), mapdn_step_record=(_STEP[:-1] + [_vp, _i64, _vp], _i32),
+    mapdn_obs_compact_layout=([_vp] * 4, _i32), mapdn_record_layout=([_vp] * 3, _i32),
+    mapdn_record=([_vp, _vp, _i64, _vp], _i32), mapdn_get_obs=([_vp] * 3, _i32), mapdn_get_state=([_vp] * 3, _i32),
+    mapdn_get_field=([_vp, _i32, _vp, _vp], _i32), mapdn_solve=([_vp, _i32] + [_vp] * 12, _i32),
+    mapdn_droop=([_vp, _i32] + [_vp] * 5 + [C.c_double, C.c_double, _i32] + [_vp] * 5, _i32),
+    mapdn_get_ybus_dense=([_vp] * 3, _i32))
+EXPORTS = tuple(SIGNATURES)
 # tester record row blocks, in the reference tester's key order (utilities/tester.py:26-32); mapdn_record_layout
 RECORD_KEYS = ("pv_active", "pv_reactive", "bus_active", "bus_reactive", "bus_voltage", "line_loss")
 
@@ -80,6 +94,15 @@ class MapdnError(RuntimeError):
     pass
 
 
+def bind(L: C.CDLL, skip_missing: bool = False) -> C.CDLL:
+    """Sets argtypes and restype of every entry point in ``L``; ``skip_missing``: pass over the symbols ``L`` lacks."""
+    for name, (argtypes, restype) in SIGNATURES.items():
+        if hasattr(L, name) or not skip_missing:
+            fn = getattr(L, name)
+            fn.argtypes, fn.restype = argtypes, restype
+    return L
+
+
 def lib() -> C.CDLL:
     """Load ``libmapdn_b200.so`` (built by ``python -m mapdn_b200.build``). Fails loudly."""
     global _lib
@@ -88,45 +111,8 @@ def lib() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise MapdnError(f"{LIB_PATH} not found - build it with `python -m mapdn_b200.build` "
                          "(there is no CPU fallback)")
-    L = C.CDLL(LIB_PATH)
-    vp = C.c_void_p
-    L.mapdn_abi_version.restype = C.c_int32
-    L.mapdn_last_error.restype = C.c_char_p
-    L.mapdn_create.argtypes = [C.POINTER(NetDescC), C.POINTER(ProfileDescC), C.POINTER(CfgC), C.c_int32,
-                               C.POINTER(vp)]
-    L.mapdn_destroy.argtypes = [vp]
-    L.mapdn_get_dims.argtypes = [vp, C.POINTER(DimsC)]
-    L.mapdn_reset.argtypes = [vp, vp, vp, C.c_int32, vp, vp, vp, vp]
-    L.mapdn_step.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, vp]
-    L.mapdn_step_host.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, vp]
-    L.mapdn_step_f32obs.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, vp]
-    L.mapdn_step_host_f32obs.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, vp]
-    dev_override = bool(os.environ.get("MAPDN_B200_LIB"))       # A/B runs against libraries built from older commits
-    try:
-        L.mapdn_step_host_pinned.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp]
-        L.mapdn_wait.argtypes = [vp, vp]
-        L.mapdn_droop.argtypes = [vp, C.c_int32] + [vp] * 5 + [C.c_double, C.c_double, C.c_int32] + [vp] * 5
-        L.mapdn_obs_compact_layout.argtypes = [vp, vp, vp, vp]
-        L.mapdn_step_host_compact.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp]
-        L.mapdn_record_layout.argtypes = [vp, vp, vp]
-        L.mapdn_record.argtypes = [vp, vp, C.c_int64, vp]
-        L.mapdn_step_record.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, vp, C.c_int64, vp]
-    except AttributeError:
-        if not dev_override:
-            raise
-    L.mapdn_get_obs.argtypes = [vp, vp, vp]
-    L.mapdn_get_state.argtypes = [vp, vp, vp]
-    L.mapdn_get_field.argtypes = [vp, C.c_int32, vp, vp]
-    L.mapdn_solve.argtypes = [vp, C.c_int32] + [vp] * 11 + [vp]
-    L.mapdn_get_ybus_dense.argtypes = [vp, vp, vp]
-    L.mapdn_launch_count.argtypes = [vp]
-    L.mapdn_launch_count.restype = C.c_int64
-    for name in EXPORTS:
-        if dev_override and not hasattr(L, name):
-            continue
-        fn = getattr(L, name)
-        if fn.restype is C.c_int and name not in ("mapdn_abi_version",):
-            fn.restype = C.c_int32
+    # MAPDN_B200_LIB: A/B runs against libraries built from older commits, which may lack the newer entry points
+    L = bind(C.CDLL(LIB_PATH), skip_missing=bool(os.environ.get("MAPDN_B200_LIB")))
     if L.mapdn_abi_version() != ABI_VERSION:
         raise MapdnError("ABI version mismatch between _capi.py and libmapdn_b200.so")
     _lib = L
@@ -155,6 +141,20 @@ def make_net_desc(net: NetDesc):
                  _p(net.bus_zone, _pi), _p(net.load_bus, _pi), _p(net.load_scaling, _pd),
                  _p(net.sgen_bus, _pi), _p(net.sgen_zone, _pi), _p(net.sgen_scaling, _pd))
     return d, keep
+
+
+def make_cfg(args: dict, batch: int, env_id_offset=0, lanes_per_env=0, tol=0.0, max_iter=0) -> CfgC:
+    """The ``mapdn_cfg`` of ``batch`` envs from the reference's ``env_args`` (every key of ``DEFAULT_ENV_ARGS``)."""
+    a, qw, lw = args, args["q_weight"], args["line_weight"]
+    return CfgC(batch=int(batch), barrier=BARRIERS[a["voltage_barrier_type"]],
+                voltage_weight=float(a["voltage_weight"]), q_weight=float(qw if qw is not None else 0.0),
+                line_weight=float(lw or 0.0), use_line_weight=int(lw is not None), v_upper=float(a["v_upper"]),
+                v_lower=float(a["v_lower"]), episode_limit=int(a["episode_limit"]),
+                action_low=float(-a["action_scale"] + a["action_bias"]),
+                action_high=float(a["action_scale"] + a["action_bias"]), reset_action=int(bool(a["reset_action"])),
+                seed=int(a["seed"]) & 0xFFFFFFFFFFFFFFFF, env_id_offset=int(env_id_offset), tol=float(tol),
+                max_iter=int(max_iter), lanes_per_env=int(lanes_per_env),
+                state_space_mask=sum(STATE_SPACE_BITS[k] for k in set(a["state_space"])))
 
 
 def make_profile_desc(prof: ProfileDesc):

@@ -233,33 +233,26 @@ std::vector<T> vec_or(const T* p, size_t n, T fill) {
 using KernelFn = void (*)(const Params);
 constexpr int kHelperPairsPerWarp = 256;   // Box-Muller pairs of a CTA round per helper warp
 
-template <int G>
+template <int G, bool DENSE>
 KernelFn kernel_for_mode(int mode, bool record) {
   switch (mode) {
-    case MODE_SOLVE: return env_kernel<G, MODE_SOLVE>;
-    case MODE_STEP: return record ? env_kernel<G, MODE_STEP, false, true> : env_kernel<G, MODE_STEP>;
-    case MODE_DROOP: return env_kernel<G, MODE_DROOP>;
-    default: return env_kernel<G, MODE_RESET>;
+    case MODE_SOLVE: return env_kernel<G, MODE_SOLVE, DENSE>;
+    case MODE_STEP: return record ? env_kernel<G, MODE_STEP, DENSE, true> : env_kernel<G, MODE_STEP, DENSE>;
+    case MODE_DROOP: return env_kernel<G, MODE_DROOP, DENSE>;
+    default: return env_kernel<G, MODE_RESET, DENSE>;
   }
 }
 
 // record: the MODE_STEP instantiation that also writes the tester record rows (mapdn_step_record)
 KernelFn kernel_for(int G, int mode, bool dense = false, bool record = false) {
-  if (dense) {
-    switch (mode) {
-      case MODE_SOLVE: return env_kernel<32, MODE_SOLVE, true>;
-      case MODE_STEP: return record ? env_kernel<32, MODE_STEP, true, true> : env_kernel<32, MODE_STEP, true>;
-      case MODE_DROOP: return env_kernel<32, MODE_DROOP, true>;
-      default: return env_kernel<32, MODE_RESET, true>;
-    }
-  }
+  if (dense) return kernel_for_mode<32, true>(mode, record);
   switch (G) {
-    case 4: return kernel_for_mode<4>(mode, record);
-    case 8: return kernel_for_mode<8>(mode, record);
-    case 16: return kernel_for_mode<16>(mode, record);
-    case 64: return kernel_for_mode<64>(mode, record);
-    case 128: return kernel_for_mode<128>(mode, record);
-    default: return kernel_for_mode<32>(mode, record);
+    case 4: return kernel_for_mode<4, false>(mode, record);
+    case 8: return kernel_for_mode<8, false>(mode, record);
+    case 16: return kernel_for_mode<16, false>(mode, record);
+    case 64: return kernel_for_mode<64, false>(mode, record);
+    case 128: return kernel_for_mode<128, false>(mode, record);
+    default: return kernel_for_mode<32, false>(mode, record);
   }
 }
 
@@ -316,6 +309,80 @@ mapdn_status launch_env_kernel(mapdn_env* e, int mode, Params& p, cudaStream_t s
     fprintf(stderr, "\n");
   }
 #endif
+  return MAPDN_OK;
+}
+
+constexpr auto nothing = [](cudaStream_t) { return MAPDN_OK; };   // before / after of a step that needs neither
+
+// The MODE_STEP launch behind the seven mapdn_step* entry points, after each has checked its own pointers: refuses a
+// handle without a profile store, then runs on the handle's device. The kernel reads the actions from and writes its
+// outputs to the given buffers (info / obs / record may be NULL; obs holds floats when obs_f32). before(st) runs ahead of
+// the launch and may refuse the call or enqueue what the kernel reads; after(st) enqueues what follows the kernel.
+template <class Before, class After>
+mapdn_status step(mapdn_env* e, const double* actions, int32_t add_noise, double* reward, uint8_t* term, double* info,
+                  void* obs, bool obs_f32, void* stream, Before before, After after, int obs_skip_off = -1,
+                  int obs_compact_len = 0, double* record = nullptr, int64_t record_stride = 0) {
+  if (!e->base.prof_pv) return fail(MAPDN_ERR_INVALID, "handle was created without a profile store");
+  MAPDN_ON_DEVICE(e->device);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  mapdn_status s = before(st);
+  if (s != MAPDN_OK) return s;
+  Params p = e->base;
+  p.actions = actions; p.add_noise = add_noise; p.reward = reward; p.term = term; p.info = info;
+  p.obs = obs_f32 ? nullptr : static_cast<double*>(obs); p.obs32 = obs_f32 ? static_cast<float*>(obs) : nullptr;
+  p.obs_skip_off = obs_skip_off; p.obs_compact_len = obs_compact_len; p.record = record; p.record_stride = record_stride;
+  s = launch_env_kernel(e, MODE_STEP, p, st);
+  return s != MAPDN_OK ? s : after(st);
+}
+
+// mapdn_step_host / mapdn_step_host_f32obs: H2D of the actions, the step into the staging buffers, D2H of the outputs
+// asked for, stream synchronisation. The fp64 staging buffer of the observations also holds them as floats.
+mapdn_status step_staged(mapdn_env* e, const double* actions_host, int32_t add_noise, double* reward_host,
+                         uint8_t* terminated_host, double* info_host, void* obs_host, bool obs_f32, void* stream) {
+  if (!e || !actions_host || !reward_host || !terminated_host) return fail(MAPDN_ERR_INVALID, "null argument");
+  const size_t B = e->dims.batch, ng = e->dims.n_sgen;
+  const size_t obs_bytes = B * ng * e->dims.obs_dim * (obs_f32 ? sizeof(float) : sizeof(double));
+  auto h2d = [&](cudaStream_t st) {
+    MAPDN_CUDA(cudaMemcpyAsync(e->d_stage_actions, actions_host, B * ng * sizeof(double), cudaMemcpyHostToDevice, st));
+    return MAPDN_OK;
+  };
+  auto d2h = [&](cudaStream_t st) {
+    MAPDN_CUDA(cudaMemcpyAsync(reward_host, e->d_stage_reward, B * sizeof(double), cudaMemcpyDeviceToHost, st));
+    MAPDN_CUDA(cudaMemcpyAsync(terminated_host, e->d_stage_term, B, cudaMemcpyDeviceToHost, st));
+    if (info_host) MAPDN_CUDA(cudaMemcpyAsync(info_host, e->d_stage_info, B * MAPDN_N_INFO * sizeof(double), cudaMemcpyDeviceToHost, st));
+    if (obs_host) MAPDN_CUDA(cudaMemcpyAsync(obs_host, e->d_stage_obs, obs_bytes, cudaMemcpyDeviceToHost, st));
+    MAPDN_CUDA(cudaStreamSynchronize(st));
+    return MAPDN_OK;
+  };
+  return step(e, e->d_stage_actions, add_noise, e->d_stage_reward, e->d_stage_term, info_host ? e->d_stage_info : nullptr,
+              obs_host ? e->d_stage_obs : nullptr, obs_f32, stream, h2d, d2h);
+}
+
+// The kernel of the pinned and compact paths reads and writes the host buffers themselves: each must be page-locked host
+// memory with unified addressing (device address = host address). Buffers that passed are remembered.
+mapdn_status check_pinned(mapdn_env* e, const void* const (&host)[5]) {
+  static const char* const what[5] = {"actions_host", "reward_host", "terminated_host", "info_host", "obs_host"};
+  for (int k = 0; k < 5; ++k) {
+    if (!host[k] || std::find(e->pinned_ok.begin(), e->pinned_ok.end(), host[k]) != e->pinned_ok.end()) continue;
+    cudaPointerAttributes at{};
+    if (cudaPointerGetAttributes(&at, host[k]) != cudaSuccess || at.type != cudaMemoryTypeHost || at.devicePointer != host[k]) {
+      cudaGetLastError();
+      return fail(MAPDN_ERR_INVALID, std::string(what[k]) + ": not page-locked host memory with unified addressing "
+                                     "(cudaHostAlloc / cudaHostRegister it, or use mapdn_step_host)");
+    }
+    if (e->pinned_ok.size() < 64) e->pinned_ok.push_back(host[k]);
+  }
+  return MAPDN_OK;
+}
+
+// One flat gather launch over n items in 256-thread blocks, on the handle's device, counted with its launches
+template <class Kernel, class... Args>
+mapdn_status gather(mapdn_env* e, Kernel kernel, long long n, void* stream, Args... args) {
+  if (n == 0) return MAPDN_OK;
+  MAPDN_ON_DEVICE(e->device);
+  MAPDN_LAUNCH(kernel, static_cast<unsigned>((n + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream), args...);
+  MAPDN_CUDA(cudaGetLastError());
+  e->launches++;
   return MAPDN_OK;
 }
 
@@ -509,8 +576,7 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
     for (int i = 0; i < npq; ++i) while (depth[order[i]] > d) dlev[++d] = static_cast<uint16_t>(i);
     while (d < n_lev) dlev[++d] = static_cast<uint16_t>(npq);
   }
-  int max_width = 0, max_children = 0;
-  for (int l = 0; l < n_lev; ++l) max_width = std::max(max_width, elev[l + 1] - elev[l]);
+  int max_children = 0;
   for (int i = 0; i < npq; ++i) max_children = std::max(max_children, nchild[i]);
   int G = cfg->lanes_per_env;
   if (G == 0) G = (npq <= 64) ? 8 : (npq <= 256 ? 32 : 64);      // fastest on H100 at every BASELINE size (DESIGN.md §4)
@@ -794,34 +860,34 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
   std::vector<unsigned> obs_src(static_cast<size_t>(ng) * obs_dim, 0u);
   std::vector<int> obs_xptr(static_cast<size_t>(ng) * obs_dim + 1, 0), obs_xidx;
   std::vector<int> agent_len(ng, 0);
-  enum { K_ZERO = 0, K_P = 1, K_Q = 2, K_PV = 3, K_QSG = 4, K_VM = 5, K_VA = 6 };
+  auto src = [](ObsKind kind, int ix) { return (static_cast<unsigned>(kind) << 28) | static_cast<unsigned>(ix); };
   for (int a = 0; a < ng; ++a) {
     // entry list of this agent in the reference's order (:254-266), then zero padding (:270-274)
-    std::vector<std::pair<unsigned, int>> ent;           // (kind, bus or sgen)
-    if (ss_dem) { for (int b : zb[a]) ent.push_back({K_P, b}); for (int b : zb[a]) ent.push_back({K_Q, b}); }
-    if (ss_pv) ent.push_back({K_PV, a});
-    if (ss_q) ent.push_back({K_QSG, a});
-    if (ss_vm) for (int b : zb[a]) ent.push_back({K_VM, b});
-    if (ss_va) for (int b : zb[a]) ent.push_back({K_VA, b});
+    std::vector<std::pair<ObsKind, int>> ent;            // (kind, bus or sgen)
+    if (ss_dem) { for (int b : zb[a]) ent.push_back({OBS_P, b}); for (int b : zb[a]) ent.push_back({OBS_Q, b}); }
+    if (ss_pv) ent.push_back({OBS_PV, a});
+    if (ss_q) ent.push_back({OBS_QSG, a});
+    if (ss_vm) for (int b : zb[a]) ent.push_back({OBS_VM, b});
+    if (ss_va) for (int b : zb[a]) ent.push_back({OBS_VA, b});
     agent_len[a] = static_cast<int>(ent.size());
     for (int k = 0; k < obs_dim; ++k) {
       const size_t idx = static_cast<size_t>(a) * obs_dim + k;
       obs_xptr[idx] = static_cast<int>(obs_xidx.size());
-      unsigned kind = K_ZERO, ix = 0;
-      int off = 2 * (npq * kNodeArrays2 + A_UP);               // sentinel record's UP.x: constant zero
+      ObsKind kind = OBS_ZERO;
+      int ix = 0, off = 2 * (npq * kNodeArrays2 + A_UP);               // sentinel record's UP.x: constant zero
       if (k < static_cast<int>(ent.size())) {
         kind = ent[k].first;
         const int t2 = ent[k].second;
-        if (kind == K_P || kind == K_Q) {
-          ix = static_cast<unsigned>(node_of_bus[t2]);
-          off = 2 * (node_of_bus[t2] * kNodeArrays2 + A_OP) + (kind == K_P ? 0 : 1);
+        if (kind == OBS_P || kind == OBS_Q) {
+          ix = node_of_bus[t2];
+          off = 2 * (node_of_bus[t2] * kNodeArrays2 + A_OP) + (kind == OBS_P ? 0 : 1);
           for (int j = 0; j < ng; ++j)
             if (net->sgen_zone[j] == net->sgen_zone[a] && net->sgen_bus[j] == t2) obs_xidx.push_back(j);
-        } else if (kind == K_PV) { ix = t2; off = 2 * pvq_off2 + t2; }
-        else if (kind == K_QSG) { ix = t2; off = 2 * pvq_off2 + ng + t2; }
-        else { ix = static_cast<unsigned>(node_of_bus[t2]); off = 2 * (node_of_bus[t2] * kNodeArrays2 + A_VV) + (kind == K_VM ? 0 : 1); }
+        } else if (kind == OBS_PV) { ix = t2; off = 2 * pvq_off2 + t2; }
+        else if (kind == OBS_QSG) { ix = t2; off = 2 * pvq_off2 + ng + t2; }
+        else { ix = node_of_bus[t2]; off = 2 * (node_of_bus[t2] * kNodeArrays2 + A_VV) + (kind == OBS_VM ? 0 : 1); }
       }
-      obs_src[idx] = (kind << 28) | ix;
+      obs_src[idx] = src(kind, ix);
       obs_off[idx] = static_cast<uint16_t>(off);
     }
   }
@@ -837,11 +903,11 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
   while (obs_compact.size() % 4) obs_compact.push_back(static_cast<uint16_t>(2 * (npq * kNodeArrays2 + A_UP)));
   // state program (reference get_state :213-230), bus-indexed
   std::vector<unsigned> state_src;
-  if (ss_dem) { for (int b = 0; b < n; ++b) state_src.push_back((7u << 28) | b); for (int b = 0; b < n; ++b) state_src.push_back((8u << 28) | b); }
-  if (ss_pv) for (int j = 0; j < ng; ++j) state_src.push_back((static_cast<unsigned>(K_PV) << 28) | j);
-  if (ss_q) for (int j = 0; j < ng; ++j) state_src.push_back((static_cast<unsigned>(K_QSG) << 28) | j);
-  if (ss_vm) for (int b = 0; b < n; ++b) state_src.push_back((static_cast<unsigned>(K_VM) << 28) | b);
-  if (ss_va) for (int b = 0; b < n; ++b) state_src.push_back((9u << 28) | b);
+  if (ss_dem) { for (int b = 0; b < n; ++b) state_src.push_back(src(OBS_PBUS, b)); for (int b = 0; b < n; ++b) state_src.push_back(src(OBS_QBUS, b)); }
+  if (ss_pv) for (int j = 0; j < ng; ++j) state_src.push_back(src(OBS_PV, j));
+  if (ss_q) for (int j = 0; j < ng; ++j) state_src.push_back(src(OBS_QSG, j));
+  if (ss_vm) for (int b = 0; b < n; ++b) state_src.push_back(src(OBS_VM, b));
+  if (ss_va) for (int b = 0; b < n; ++b) state_src.push_back(src(OBS_VA_DEG, b));
   const int state_dim = static_cast<int>(state_src.size());
 
   // ---- 3a. line-loss table + scaling ----
@@ -1199,7 +1265,6 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
   d.lanes_per_env = G; d.envs_per_block = e->epb; d.smem_bytes = e->smem; d.n_levels = n_lev;
   // SURVEY §8d: read p_load,q_load,p_pv,a ; write vm,va ; write obs ; reward+done+11 info
   d.algorithmic_bytes_per_env_step = 8LL * (2 * nl + 2 * ng) + 8LL * 2 * n + 8LL * ng * obs_dim + 8LL * 13;
-  (void)max_width;
   // the memsets / uploads above ran on the legacy default stream: order them before any launch of the caller's
   // (possibly non-blocking) streams
   TRY_CUDA(cudaDeviceSynchronize());
@@ -1231,12 +1296,7 @@ mapdn_status mapdn_reset(mapdn_env* e, const int32_t* start_dhi_dev, const uint8
 mapdn_status mapdn_step(mapdn_env* e, const double* actions_dev, int32_t add_noise, double* reward_dev,
                         uint8_t* terminated_dev, double* info_dev, double* obs_dev, void* stream) {
   if (!e || !actions_dev || !reward_dev || !terminated_dev) return fail(MAPDN_ERR_INVALID, "null argument");
-  if (!e->base.prof_pv) return fail(MAPDN_ERR_INVALID, "handle was created without a profile store");
-  MAPDN_ON_DEVICE(e->device);
-  Params p = e->base;
-  p.actions = actions_dev; p.add_noise = add_noise; p.reward = reward_dev; p.term = terminated_dev;
-  p.info = info_dev; p.obs = obs_dev;
-  return launch_env_kernel(e, MODE_STEP, p, static_cast<cudaStream_t>(stream));
+  return step(e, actions_dev, add_noise, reward_dev, terminated_dev, info_dev, obs_dev, false, stream, nothing, nothing);
 }
 
 static int record_row_len(const mapdn_env* e) { return 2 * e->dims.n_sgen + 3 * e->dims.n_bus + e->dims.n_line; }
@@ -1253,86 +1313,39 @@ mapdn_status mapdn_record_layout(const mapdn_env* e, int32_t* off, int32_t* row_
 mapdn_status mapdn_record(mapdn_env* e, double* record_dev, int64_t record_stride, void* stream) {
   if (!e || !record_dev) return fail(MAPDN_ERR_INVALID, "null argument");
   if (record_stride < record_row_len(e)) return fail(MAPDN_ERR_INVALID, "record_stride shorter than a record row");
-  MAPDN_ON_DEVICE(e->device);
   Params p = e->base;
   p.record = record_dev; p.record_stride = record_stride;
-  const long long tot = static_cast<long long>(p.nb) * record_row_len(e);
-  MAPDN_LAUNCH(record_kernel, static_cast<unsigned>((tot + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream), p);
-  MAPDN_CUDA(cudaGetLastError());
-  e->launches++;
-  return MAPDN_OK;
+  return gather(e, record_kernel, static_cast<long long>(p.nb) * record_row_len(e), stream, p);
 }
 
 mapdn_status mapdn_step_record(mapdn_env* e, const double* actions_dev, int32_t add_noise, double* reward_dev,
                                uint8_t* terminated_dev, double* info_dev, double* obs_dev, double* record_dev,
                                int64_t record_stride, void* stream) {
   if (!e || !actions_dev || !reward_dev || !terminated_dev) return fail(MAPDN_ERR_INVALID, "null argument");
-  if (!e->base.prof_pv) return fail(MAPDN_ERR_INVALID, "handle was created without a profile store");
-  if (record_dev && record_stride < record_row_len(e)) return fail(MAPDN_ERR_INVALID, "record_stride shorter than a record row");
-  MAPDN_ON_DEVICE(e->device);
-  Params p = e->base;
-  p.actions = actions_dev; p.add_noise = add_noise; p.reward = reward_dev; p.term = terminated_dev;
-  p.info = info_dev; p.obs = obs_dev;
-  p.record = record_dev; p.record_stride = record_stride;
-  return launch_env_kernel(e, MODE_STEP, p, static_cast<cudaStream_t>(stream));
+  auto check_stride = [&](cudaStream_t) {
+    if (record_dev && record_stride < record_row_len(e)) return fail(MAPDN_ERR_INVALID, "record_stride shorter than a record row");
+    return MAPDN_OK;
+  };
+  return step(e, actions_dev, add_noise, reward_dev, terminated_dev, info_dev, obs_dev, false, stream, check_stride, nothing,
+              -1, 0, record_dev, record_stride);
 }
 
 mapdn_status mapdn_step_host(mapdn_env* e, const double* actions_host, int32_t add_noise, double* reward_host,
                              uint8_t* terminated_host, double* info_host, double* obs_host, void* stream) {
-  if (!e || !actions_host || !reward_host || !terminated_host) return fail(MAPDN_ERR_INVALID, "null argument");
-  MAPDN_ON_DEVICE(e->device);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const size_t B = e->dims.batch, ng = e->dims.n_sgen, od = e->dims.obs_dim;
-  MAPDN_CUDA(cudaMemcpyAsync(e->d_stage_actions, actions_host, B * ng * sizeof(double), cudaMemcpyHostToDevice, st));
-  mapdn_status s = mapdn_step(e, e->d_stage_actions, add_noise, e->d_stage_reward, e->d_stage_term, info_host ? e->d_stage_info : nullptr,
-                              obs_host ? e->d_stage_obs : nullptr, stream);
-  if (s != MAPDN_OK) return s;
-  MAPDN_CUDA(cudaMemcpyAsync(reward_host, e->d_stage_reward, B * sizeof(double), cudaMemcpyDeviceToHost, st));
-  MAPDN_CUDA(cudaMemcpyAsync(terminated_host, e->d_stage_term, B, cudaMemcpyDeviceToHost, st));
-  if (info_host) MAPDN_CUDA(cudaMemcpyAsync(info_host, e->d_stage_info, B * MAPDN_N_INFO * sizeof(double), cudaMemcpyDeviceToHost, st));
-  if (obs_host) MAPDN_CUDA(cudaMemcpyAsync(obs_host, e->d_stage_obs, B * ng * od * sizeof(double), cudaMemcpyDeviceToHost, st));
-  MAPDN_CUDA(cudaStreamSynchronize(st));
-  return MAPDN_OK;
-}
-
-// device alias of a pinned host buffer (unified addressing); verified once per buffer
-static mapdn_status pinned_alias(mapdn_env* e, const void* host, void** dev, const char* what) {
-  *dev = const_cast<void*>(host);
-  if (!host) return MAPDN_OK;
-  if (std::find(e->pinned_ok.begin(), e->pinned_ok.end(), host) != e->pinned_ok.end()) return MAPDN_OK;
-  cudaPointerAttributes at{};
-  if (cudaPointerGetAttributes(&at, host) != cudaSuccess || at.type != cudaMemoryTypeHost || at.devicePointer != host) {
-    cudaGetLastError();
-    return fail(MAPDN_ERR_INVALID, std::string(what) + ": not page-locked host memory with unified addressing "
-                                   "(cudaHostAlloc / cudaHostRegister it, or use mapdn_step_host)");
-  }
-  if (e->pinned_ok.size() < 64) e->pinned_ok.push_back(host);
-  return MAPDN_OK;
+  return step_staged(e, actions_host, add_noise, reward_host, terminated_host, info_host, obs_host, false, stream);
 }
 
 mapdn_status mapdn_step_host_pinned(mapdn_env* e, const double* actions_host, int32_t add_noise, double* reward_host,
                                     uint8_t* terminated_host, double* info_host, void* obs_host, int32_t obs_is_f32,
                                     int32_t skip_padding, int32_t sync, void* stream) {
   if (!e || !actions_host || !reward_host || !terminated_host) return fail(MAPDN_ERR_INVALID, "null argument");
-  if (!e->base.prof_pv) return fail(MAPDN_ERR_INVALID, "handle was created without a profile store");
-  MAPDN_ON_DEVICE(e->device);
-  void *a, *r, *t, *i, *o;
-  mapdn_status s;
-  if ((s = pinned_alias(e, actions_host, &a, "actions_host")) != MAPDN_OK) return s;
-  if ((s = pinned_alias(e, reward_host, &r, "reward_host")) != MAPDN_OK) return s;
-  if ((s = pinned_alias(e, terminated_host, &t, "terminated_host")) != MAPDN_OK) return s;
-  if ((s = pinned_alias(e, info_host, &i, "info_host")) != MAPDN_OK) return s;
-  if ((s = pinned_alias(e, obs_host, &o, "obs_host")) != MAPDN_OK) return s;
-  Params p = e->base;
-  p.actions = static_cast<const double*>(a); p.add_noise = add_noise; p.reward = static_cast<double*>(r);
-  p.term = static_cast<unsigned char*>(t); p.info = static_cast<double*>(i);
-  p.obs = obs_is_f32 ? nullptr : static_cast<double*>(o);
-  p.obs32 = obs_is_f32 ? static_cast<float*>(o) : nullptr;
-  p.obs_skip_off = skip_padding ? e->obs_zero_off : -1;
-  s = launch_env_kernel(e, MODE_STEP, p, static_cast<cudaStream_t>(stream));
-  if (s != MAPDN_OK) return s;
-  if (sync) MAPDN_CUDA(cudaStreamSynchronize(static_cast<cudaStream_t>(stream)));
-  return MAPDN_OK;
+  auto pinned = [&](cudaStream_t) { return check_pinned(e, {actions_host, reward_host, terminated_host, info_host, obs_host}); };
+  auto finish = [&](cudaStream_t st) {
+    if (sync) MAPDN_CUDA(cudaStreamSynchronize(st));
+    return MAPDN_OK;
+  };
+  return step(e, actions_host, add_noise, reward_host, terminated_host, info_host, obs_host, obs_is_f32, stream, pinned, finish,
+              skip_padding ? e->obs_zero_off : -1);
 }
 
 mapdn_status mapdn_obs_compact_layout(const mapdn_env* e, int32_t* agent_off, int32_t* agent_len, int32_t* row_len) {
@@ -1349,31 +1362,16 @@ mapdn_status mapdn_step_host_compact(mapdn_env* e, const double* actions_host, i
                                      uint8_t* terminated_host, double* info_host, void* obs_host, int32_t obs_is_f32,
                                      int32_t direct, int32_t sync, void* stream) {
   if (!e || !actions_host || !reward_host || !terminated_host || !obs_host) return fail(MAPDN_ERR_INVALID, "null argument");
-  if (!e->base.prof_pv) return fail(MAPDN_ERR_INVALID, "handle was created without a profile store");
-  MAPDN_ON_DEVICE(e->device);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  void *a, *r, *t, *i, *o;
-  mapdn_status s;
-  if ((s = pinned_alias(e, actions_host, &a, "actions_host")) != MAPDN_OK) return s;
-  if ((s = pinned_alias(e, reward_host, &r, "reward_host")) != MAPDN_OK) return s;
-  if ((s = pinned_alias(e, terminated_host, &t, "terminated_host")) != MAPDN_OK) return s;
-  if ((s = pinned_alias(e, info_host, &i, "info_host")) != MAPDN_OK) return s;
-  if ((s = pinned_alias(e, obs_host, &o, "obs_host")) != MAPDN_OK) return s;    // pageable memory would make the copy synchronous
-  Params p = e->base;
-  p.actions = static_cast<const double*>(a); p.add_noise = add_noise; p.reward = static_cast<double*>(r);
-  p.term = static_cast<unsigned char*>(t); p.info = static_cast<double*>(i);
-  void* dst = direct ? o : static_cast<void*>(e->d_stage_obs);
-  p.obs = obs_is_f32 ? nullptr : static_cast<double*>(dst);
-  p.obs32 = obs_is_f32 ? static_cast<float*>(dst) : nullptr;
-  p.obs_compact_len = e->compact_row;
-  s = launch_env_kernel(e, MODE_STEP, p, st);
-  if (s != MAPDN_OK) return s;
-  if (!direct) {
+  // obs_host is checked also when the rows go through the staging buffer: a copy to pageable memory would be synchronous
+  auto pinned = [&](cudaStream_t) { return check_pinned(e, {actions_host, reward_host, terminated_host, info_host, obs_host}); };
+  auto finish = [&](cudaStream_t st) {
     const size_t bytes = static_cast<size_t>(e->dims.batch) * e->compact_row * (obs_is_f32 ? sizeof(float) : sizeof(double));
-    MAPDN_CUDA(cudaMemcpyAsync(obs_host, e->d_stage_obs, bytes, cudaMemcpyDeviceToHost, st));
-  }
-  if (sync) MAPDN_CUDA(cudaStreamSynchronize(st));
-  return MAPDN_OK;
+    if (!direct) MAPDN_CUDA(cudaMemcpyAsync(obs_host, e->d_stage_obs, bytes, cudaMemcpyDeviceToHost, st));
+    if (sync) MAPDN_CUDA(cudaStreamSynchronize(st));
+    return MAPDN_OK;
+  };
+  return step(e, actions_host, add_noise, reward_host, terminated_host, info_host, direct ? obs_host : e->d_stage_obs,
+              obs_is_f32, stream, pinned, finish, -1, e->compact_row);
 }
 
 mapdn_status mapdn_wait(mapdn_env* e, void* stream) {
@@ -1386,61 +1384,30 @@ mapdn_status mapdn_wait(mapdn_env* e, void* stream) {
 mapdn_status mapdn_step_f32obs(mapdn_env* e, const double* actions_dev, int32_t add_noise, double* reward_dev,
                                uint8_t* terminated_dev, double* info_dev, float* obs_dev, void* stream) {
   if (!e || !actions_dev || !reward_dev || !terminated_dev) return fail(MAPDN_ERR_INVALID, "null argument");
-  if (!e->base.prof_pv) return fail(MAPDN_ERR_INVALID, "handle was created without a profile store");
-  MAPDN_ON_DEVICE(e->device);
-  Params p = e->base;
-  p.actions = actions_dev; p.add_noise = add_noise; p.reward = reward_dev; p.term = terminated_dev;
-  p.info = info_dev; p.obs = nullptr; p.obs32 = obs_dev;
-  return launch_env_kernel(e, MODE_STEP, p, static_cast<cudaStream_t>(stream));
+  return step(e, actions_dev, add_noise, reward_dev, terminated_dev, info_dev, obs_dev, true, stream, nothing, nothing);
 }
 
 mapdn_status mapdn_step_host_f32obs(mapdn_env* e, const double* actions_host, int32_t add_noise, double* reward_host,
                                     uint8_t* terminated_host, double* info_host, float* obs_host, void* stream) {
-  if (!e || !actions_host || !reward_host || !terminated_host) return fail(MAPDN_ERR_INVALID, "null argument");
-  MAPDN_ON_DEVICE(e->device);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const size_t B = e->dims.batch, ng = e->dims.n_sgen, od = e->dims.obs_dim;
-  float* d_obs32 = reinterpret_cast<float*>(e->d_stage_obs);          // the fp64 staging buffer is large enough
-  MAPDN_CUDA(cudaMemcpyAsync(e->d_stage_actions, actions_host, B * ng * sizeof(double), cudaMemcpyHostToDevice, st));
-  mapdn_status s = mapdn_step_f32obs(e, e->d_stage_actions, add_noise, e->d_stage_reward, e->d_stage_term,
-                                     info_host ? e->d_stage_info : nullptr, obs_host ? d_obs32 : nullptr, stream);
-  if (s != MAPDN_OK) return s;
-  MAPDN_CUDA(cudaMemcpyAsync(reward_host, e->d_stage_reward, B * sizeof(double), cudaMemcpyDeviceToHost, st));
-  MAPDN_CUDA(cudaMemcpyAsync(terminated_host, e->d_stage_term, B, cudaMemcpyDeviceToHost, st));
-  if (info_host) MAPDN_CUDA(cudaMemcpyAsync(info_host, e->d_stage_info, B * MAPDN_N_INFO * sizeof(double), cudaMemcpyDeviceToHost, st));
-  if (obs_host) MAPDN_CUDA(cudaMemcpyAsync(obs_host, d_obs32, B * ng * od * sizeof(float), cudaMemcpyDeviceToHost, st));
-  MAPDN_CUDA(cudaStreamSynchronize(st));
-  return MAPDN_OK;
+  return step_staged(e, actions_host, add_noise, reward_host, terminated_host, info_host, obs_host, true, stream);
 }
 
 mapdn_status mapdn_get_obs(mapdn_env* e, double* obs_dev, void* stream) {
   if (!e || !obs_dev) return fail(MAPDN_ERR_INVALID, "null argument");
-  MAPDN_ON_DEVICE(e->device);
   Params p = e->base;
   p.obs = obs_dev;
-  const long long tot = static_cast<long long>(p.nb) * p.n_sgen * p.obs_dim;
-  MAPDN_LAUNCH(get_obs_kernel, static_cast<unsigned>((tot + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream), p);
-  MAPDN_CUDA(cudaGetLastError());
-  e->launches++;
-  return MAPDN_OK;
+  return gather(e, get_obs_kernel, static_cast<long long>(p.nb) * p.n_sgen * p.obs_dim, stream, p);
 }
 
 mapdn_status mapdn_get_state(mapdn_env* e, double* state_dev, void* stream) {
   if (!e || !state_dev) return fail(MAPDN_ERR_INVALID, "null argument");
-  MAPDN_ON_DEVICE(e->device);
   Params p = e->base;
   p.state = state_dev;
-  const long long tot = static_cast<long long>(p.nb) * p.state_dim;
-  MAPDN_LAUNCH(get_state_kernel, static_cast<unsigned>((tot + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream), p);
-  MAPDN_CUDA(cudaGetLastError());
-  e->launches++;
-  return MAPDN_OK;
+  return gather(e, get_state_kernel, static_cast<long long>(p.nb) * p.state_dim, stream, p);
 }
 
 mapdn_status mapdn_get_field(mapdn_env* e, int32_t field, double* out_dev, void* stream) {
   if (!e || !out_dev) return fail(MAPDN_ERR_INVALID, "null argument");
-  MAPDN_ON_DEVICE(e->device);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   const Params& p = e->base;
   const long long B = p.nb;
   const double* src = nullptr;
@@ -1457,25 +1424,12 @@ mapdn_status mapdn_get_field(mapdn_env* e, int32_t field, double* out_dev, void*
     case MAPDN_FIELD_P_LOAD: src = p.cur_pl; cnt = B * p.n_load; break;
     case MAPDN_FIELD_Q_LOAD: src = p.cur_ql; cnt = B * p.n_load; break;
     case MAPDN_FIELD_SUM_REWARDS: src = p.sum_rewards; cnt = B; break;
-    case MAPDN_FIELD_STEPS:
-      MAPDN_LAUNCH(int_to_double_kernel, static_cast<unsigned>((B + 255) / 256), 256, 0, st, B, p.steps, out_dev);
-      MAPDN_CUDA(cudaGetLastError()); e->launches++;
-      return MAPDN_OK;
-    case MAPDN_FIELD_NR_ITERS:
-      MAPDN_LAUNCH(int_to_double_kernel, static_cast<unsigned>((B + 255) / 256), 256, 0, st, B, p.nr_iters, out_dev);
-      MAPDN_CUDA(cudaGetLastError()); e->launches++;
-      return MAPDN_OK;
-    case MAPDN_FIELD_START_ROW:
-      MAPDN_LAUNCH(i64_to_double_kernel, static_cast<unsigned>((B + 255) / 256), 256, 0, st, B, p.start_row, out_dev);
-      MAPDN_CUDA(cudaGetLastError()); e->launches++;
-      return MAPDN_OK;
+    case MAPDN_FIELD_STEPS: return gather(e, int_to_double_kernel, B, stream, B, p.steps, out_dev);
+    case MAPDN_FIELD_NR_ITERS: return gather(e, int_to_double_kernel, B, stream, B, p.nr_iters, out_dev);
+    case MAPDN_FIELD_START_ROW: return gather(e, i64_to_double_kernel, B, stream, B, p.start_row, out_dev);
     default: return fail(MAPDN_ERR_INVALID, "unknown field");
   }
-  if (cnt == 0) return MAPDN_OK;
-  MAPDN_LAUNCH(scale_copy_kernel, static_cast<unsigned>((cnt + 255) / 256), 256, 0, st, cnt, src, scale, out_dev);
-  MAPDN_CUDA(cudaGetLastError());
-  e->launches++;
-  return MAPDN_OK;
+  return gather(e, scale_copy_kernel, cnt, stream, cnt, src, scale, out_dev);
 }
 
 mapdn_status mapdn_solve(mapdn_env* e, int32_t nb, const double* p_load, const double* q_load, const double* p_sgen,

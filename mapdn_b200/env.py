@@ -76,20 +76,7 @@ class BatchedVoltageControl:
         self.device_index = torch.cuda.current_device() if device is None else int(device)
         self.device = torch.device("cuda", self.device_index)
         L = _capi.lib()
-        cfg = _capi.CfgC(
-            batch=self.batch, barrier=_capi.BARRIERS[args["voltage_barrier_type"]],
-            voltage_weight=float(args["voltage_weight"]),
-            q_weight=float(args["q_weight"] if args["q_weight"] is not None else 0.0),
-            line_weight=float(args["line_weight"] or 0.0),
-            use_line_weight=int(args["line_weight"] is not None),
-            v_upper=float(args["v_upper"]), v_lower=float(args["v_lower"]),
-            episode_limit=int(args["episode_limit"]),
-            action_low=float(-args["action_scale"] + args["action_bias"]),
-            action_high=float(args["action_scale"] + args["action_bias"]),
-            reset_action=int(bool(args["reset_action"])), seed=int(args["seed"]) & 0xFFFFFFFFFFFFFFFF,
-            env_id_offset=int(env_id_offset), tol=float(tol), max_iter=int(max_iter),
-            lanes_per_env=int(lanes_per_env),
-            state_space_mask=sum(_capi.STATE_SPACE_BITS[k] for k in set(args["state_space"])))
+        cfg = _capi.make_cfg(args, self.batch, env_id_offset, lanes_per_env, tol, max_iter)
         if args["line_weight"] is None and args["q_weight"] is None:
             raise NotImplementedError("Please at least give one weight, either q_weight or line_weight.")
         nd, keep1 = _capi.make_net_desc(net)
@@ -336,11 +323,7 @@ class BatchedVoltageControl:
         return self.state
 
     def get_field(self, name: str) -> torch.Tensor:
-        d = self.dims
-        width = dict(vm=d["n_bus"], va_deg=d["n_bus"], p_bus=d["n_bus"], q_bus=d["n_bus"], p_sgen=d["n_sgen"],
-                     q_sgen=d["n_sgen"], line_loss=d["n_line"], p_load=d["n_load"], q_load=d["n_load"],
-                     sum_rewards=1, steps=1, start_row=1, nr_iters=1)[name]
-        out = torch.empty(self.batch, width, dtype=torch.float64, device=self.device)
+        out = torch.empty(self.batch, self.dims.get(_capi.FIELD_DIMS.get(name), 1), dtype=torch.float64, device=self.device)
         _capi.check(self._L.mapdn_get_field(self._h, _capi.FIELDS[name], _ptr(out), self._stream()))
         return out
 

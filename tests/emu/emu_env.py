@@ -36,27 +36,8 @@ _L = None
 def lib():
     global _L
     if _L is None:
-        L = C.CDLL(build())
-        vp = C.c_void_p
-        L.mapdn_last_error.restype = C.c_char_p
-        L.mapdn_create.argtypes = [C.POINTER(_capi.NetDescC), C.POINTER(_capi.ProfileDescC), C.POINTER(_capi.CfgC), C.c_int32,
-                                   C.POINTER(vp)]
-        L.mapdn_destroy.argtypes = [vp]
-        L.mapdn_get_dims.argtypes = [vp, C.POINTER(_capi.DimsC)]
-        L.mapdn_reset.argtypes = [vp, vp, vp, C.c_int32, vp, vp, vp, vp]
-        L.mapdn_step.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, vp]
-        L.mapdn_get_obs.argtypes = [vp, vp, vp]
-        L.mapdn_get_state.argtypes = [vp, vp, vp]
-        L.mapdn_get_field.argtypes = [vp, C.c_int32, vp, vp]
-        L.mapdn_solve.argtypes = [vp, C.c_int32] + [vp] * 11 + [vp]
-        L.mapdn_droop.argtypes = [vp, C.c_int32] + [vp] * 5 + [C.c_double, C.c_double, C.c_int32] + [vp] * 5
-        L.mapdn_step_host.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, vp]
-        L.mapdn_step_host_f32obs.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, vp]
-        L.mapdn_step_host_pinned.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp]
-        L.mapdn_step_host_compact.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp]
-        L.mapdn_obs_compact_layout.argtypes = [vp, vp, vp, vp]
-        L.mapdn_wait.argtypes = [vp, vp]
-        _L = L
+        _L = _capi.bind(C.CDLL(build()))
+        _L.mapdn_emu_last_grid.argtypes, _L.mapdn_emu_last_grid.restype = [], C.c_int
     return _L
 
 
@@ -73,16 +54,7 @@ class EmuEnv:
         args.update(env_args or {})
         self.args, self.net, self.batch = args, net, batch
         L = lib()
-        cfg = _capi.CfgC(batch=batch, barrier=_capi.BARRIERS[args["voltage_barrier_type"]],
-                         voltage_weight=float(args["voltage_weight"]),
-                         q_weight=float(args["q_weight"] if args["q_weight"] is not None else 0.0),
-                         line_weight=float(args["line_weight"] or 0.0), use_line_weight=int(args["line_weight"] is not None),
-                         v_upper=float(args["v_upper"]), v_lower=float(args["v_lower"]), episode_limit=int(args["episode_limit"]),
-                         action_low=float(-args["action_scale"] + args["action_bias"]),
-                         action_high=float(args["action_scale"] + args["action_bias"]),
-                         reset_action=int(bool(args["reset_action"])), seed=int(args["seed"]), env_id_offset=env_id_offset,
-                         tol=0.0, max_iter=0, lanes_per_env=lanes_per_env,
-                         state_space_mask=sum(_capi.STATE_SPACE_BITS[k] for k in set(args["state_space"])))
+        cfg = _capi.make_cfg(args, batch, env_id_offset, lanes_per_env)
         nd, self._k1 = _capi.make_net_desc(net)
         pd_, self._k2 = (None, None) if prof is None else _capi.make_profile_desc(prof)
         h = C.c_void_p()
@@ -135,16 +107,30 @@ class EmuEnv:
                                    _ptr(self.obs), None))
         return self.reward, self.term, self.info
 
+    # ---- tester records (mapdn_record_layout / mapdn_record / mapdn_step_record) ----
+    def record_layout(self):
+        off, row = (C.c_int32 * 6)(), C.c_int32(0)
+        self._chk(lib().mapdn_record_layout(self._h, off, C.byref(row)))
+        return [int(o) for o in off], int(row.value)
+
+    def record(self, out):
+        """mapdn_record into ``out`` (a [B, >= row_len] fp64 array, any row stride)."""
+        self._chk(lib().mapdn_record(self._h, _ptr(out), out.strides[0] // 8, None))
+        return out
+
+    def step_record(self, actions, out, add_noise=True):
+        """mapdn_step_record: the step of :meth:`step`, plus the record row of every env in ``out``."""
+        a = np.ascontiguousarray(actions, np.float64)
+        self._chk(lib().mapdn_step_record(self._h, _ptr(a), int(add_noise), _ptr(self.reward), _ptr(self.term),
+                                          _ptr(self.info), _ptr(self.obs), _ptr(out), out.strides[0] // 8, None))
+        return self.reward, self.term, self.info
+
     def get_state(self):
         self._chk(lib().mapdn_get_state(self._h, _ptr(self.state), None))
         return self.state
 
     def get_field(self, name):
-        d = self.dims
-        width = dict(vm=d["n_bus"], va_deg=d["n_bus"], p_bus=d["n_bus"], q_bus=d["n_bus"], p_sgen=d["n_sgen"],
-                     q_sgen=d["n_sgen"], line_loss=d["n_line"], p_load=d["n_load"], q_load=d["n_load"],
-                     sum_rewards=1, steps=1, start_row=1, nr_iters=1)[name]
-        out = np.zeros((self.batch, width))
+        out = np.zeros((self.batch, self.dims.get(_capi.FIELD_DIMS.get(name), 1)))
         self._chk(lib().mapdn_get_field(self._h, _capi.FIELDS[name], _ptr(out), None))
         return out
 

@@ -23,7 +23,7 @@ from mapdn_b200 import cases
 from mapdn_b200.network import NetDesc, ProfileDesc
 
 sys.path.insert(0, os.path.join(ROOT, "tests", "emu"))
-from emu_record import EmuRecordEnv                                 # noqa: E402
+from emu_env import EmuEnv                                          # noqa: E402
 from oracle.pandapower_nr import PandapowerEquivalent               # noqa: E402
 from oracle.voltage_control_ref import INFO_KEYS, VoltageControlOracle   # noqa: E402
 from test_emu_kernel import _oracle_droop                           # noqa: E402
@@ -92,7 +92,7 @@ def run_geometry(monkeypatch, name, lanes, batch, geom, n_steps=2, seed=5, droop
     net, prof, scale = _net(name)
     _set_geometry(monkeypatch, geom)
     args = dict(voltage_barrier_type="bowl", action_scale=scale, seed=seed)
-    env = EmuRecordEnv(net, prof, args, batch=batch, lanes_per_env=lanes, env_id_offset=100)
+    env = EmuEnv(net, prof, args, batch=batch, lanes_per_env=lanes, env_id_offset=100)
     try:
         acts = GC.actions(batch, net.n_sgen, scale, n_steps, seed)
         _, R = env.record_layout()
@@ -272,7 +272,7 @@ def test_diverging_and_never_converging_envs_in_later_rounds(monkeypatch, geom, 
     start = np.array([[1, e % 24, (3 * e) % 20] for e in range(B)], np.int32)       # day 1: clear of the overload
     start[11] = (0, 2, 18)                         # row 58: the reset solves row 59, step 1 loads row 60, step 2 diverges
     _set_geometry(monkeypatch, geom)
-    env = EmuRecordEnv(net, prof, args, batch=B, env_id_offset=100)
+    env = EmuEnv(net, prof, args, batch=B, env_id_offset=100)
     d = env.dims
     ors = [VoltageControlOracle(net, prof, env.args, env_id=100 + e) for e in range(B)]
     acts = GC.actions(B, net.n_sgen, scale, 4, seed=2)
@@ -349,11 +349,11 @@ def test_meshed_case141_dense_fallback_matches_the_oracle(monkeypatch):
 def test_meshed_net_size_limit_of_the_dense_fallback(monkeypatch):
     """256 PQ buses are accepted (one warp per env, 2 npq = 512); 257 are refused at create with MAPDN_ERR_TOPOLOGY (3)."""
     _set_geometry(monkeypatch, dict(MAPDN_EMU_SMS=1))
-    env = EmuRecordEnv(GC.meshed_chain(256), None, dict(voltage_barrier_type="l1"), batch=1)
+    env = EmuEnv(GC.meshed_chain(256), None, dict(voltage_barrier_type="l1"), batch=1)
     assert env.dims["lanes_per_env"] == 32 and env.dims["n_bus"] == 257
     env.close()
     with pytest.raises(RuntimeError, match=r"mapdn status 3: .*more than 256 PQ buses"):
-        EmuRecordEnv(GC.meshed_chain(257), None, dict(voltage_barrier_type="l1"), batch=1)
+        EmuEnv(GC.meshed_chain(257), None, dict(voltage_barrier_type="l1"), batch=1)
 
 
 @pytest.mark.parametrize("lanes,cap", [(32, 8), (64, 8), (128, 4)])
@@ -362,6 +362,6 @@ def test_envs_per_block_override_is_capped(monkeypatch, lanes, cap):
     kernel's launch bounds and the named-barrier ids 3 + group): a small net whose shared memory would allow more."""
     net, prof, _ = _net("hub")
     _set_geometry(monkeypatch, dict(MAPDN_EPB=64))
-    env = EmuRecordEnv(net, prof, None, batch=64, lanes_per_env=lanes)
+    env = EmuEnv(net, prof, None, batch=64, lanes_per_env=lanes)
     assert env.dims["lanes_per_env"] == lanes and env.dims["envs_per_block"] == cap
     env.close()

@@ -13,7 +13,7 @@ from mapdn_b200 import _capi, cases
 from mapdn_b200.network import NetDesc, ProfileDesc
 
 sys.path.insert(0, os.path.join(ROOT, "tests", "emu"))
-from emu_record import EmuRecordEnv                                 # noqa: E402
+from emu_env import EmuEnv                                          # noqa: E402
 
 FIELD_ORDER = ("p_sgen", "q_sgen", "p_bus", "q_bus", "vm", "line_loss")     # = RECORD_KEYS, getter by getter
 
@@ -42,8 +42,8 @@ def _mesh():
 
 
 def _run(net, prof, args, batch, lanes, start, n_steps, noise, expect_diverged=False):
-    plain = EmuRecordEnv(net, prof, args, batch=batch, lanes_per_env=lanes)
-    fused = EmuRecordEnv(net, prof, args, batch=batch, lanes_per_env=lanes)
+    plain = EmuEnv(net, prof, args, batch=batch, lanes_per_env=lanes)
+    fused = EmuEnv(net, prof, args, batch=batch, lanes_per_env=lanes)
     off, R = fused.record_layout()
     ng, n, nl = net.n_sgen, net.n_bus, fused.dims["n_line"]
     assert off == [0, ng, 2 * ng, 2 * ng + n, 2 * ng + 2 * n, 2 * ng + 3 * n] and R == 2 * ng + 3 * n + nl
@@ -105,7 +105,7 @@ def test_record_layout_matches_the_header():
     doc = re.search(r"\[(pv_active[^\]]*)\]", src).group(1)
     assert [tok.split()[0] for tok in doc.split("|")] == list(_capi.RECORD_KEYS)
     net, prof = cases.make_case("case141"), cases.make_profiles("case141", n_days=3)
-    env = EmuRecordEnv(net, prof, None, batch=1)
+    env = EmuEnv(net, prof, None, batch=1)
     off, R = env.record_layout()
     widths = [net.n_sgen, net.n_sgen, net.n_bus, net.n_bus, net.n_bus, env.dims["n_line"]]
     assert off == list(np.cumsum([0] + widths[:-1])) and R == sum(widths)
