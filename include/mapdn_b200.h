@@ -257,6 +257,26 @@ mapdn_status mapdn_step_record(mapdn_env* env, const double* actions_dev /*[B,n_
                                double* info_dev /*[B,11] or NULL*/, double* obs_dev /*or NULL*/,
                                double* record_dev /*or NULL*/, int64_t record_stride, void* stream);
 
+/*
+ * Observation history (env_args `history`, reference :87, :303-315): with history = H > 1 every get_obs() returns each
+ * agent's last H frames side by side, oldest first, zero frames before the episode start - rows [n_agents, H*obs_dim].
+ * mapdn_set_history(H): H > 1 allocates a zero-filled frame ring on the device [B, H, n_agents*obs_dim]; from then on
+ * every reset and every step (any mapdn_step* entry point, obs requested or not) records the env's newest frame in it.
+ * Frame f of an env counts the frames since its last reset (the reset gives f = 0) and lives in slot f mod H, so a reset
+ * clears nothing. H = 1 frees the ring; H < 1 is refused.
+ * mapdn_step_stacked: mapdn_step_record (same arguments, same outputs) whose kernel also writes the stacked rows
+ * [B, n_agents, H*obs_dim] to obs_stacked_dev (may be NULL) - one launch.
+ * mapdn_get_obs_stacked: one gather launch writing the same rows from the ring (after a reset or a host-path step).
+ * Both refuse a handle without history. mapdn_dims.obs_dim stays the width of one frame.
+ */
+mapdn_status mapdn_set_history(mapdn_env* env, int32_t history);
+mapdn_status mapdn_step_stacked(mapdn_env* env, const double* actions_dev /*[B,n_sgen]*/, int32_t add_noise,
+                                double* reward_dev /*[B]*/, uint8_t* terminated_dev /*[B]*/,
+                                double* info_dev /*[B,11] or NULL*/, double* obs_dev /*or NULL*/,
+                                double* obs_stacked_dev /*[B,n_agents,H*obs_dim] or NULL*/,
+                                double* record_dev /*or NULL*/, int64_t record_stride, void* stream);
+mapdn_status mapdn_get_obs_stacked(mapdn_env* env, double* obs_stacked_dev, void* stream);
+
 mapdn_status mapdn_get_obs(mapdn_env* env, double* obs_dev, void* stream);      /* :232-316 */
 mapdn_status mapdn_get_state(mapdn_env* env, double* state_dev, void* stream);  /* :213-230 */
 mapdn_status mapdn_get_field(mapdn_env* env, int32_t field, double* out_dev, void* stream);

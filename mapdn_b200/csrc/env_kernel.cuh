@@ -12,6 +12,8 @@
 // envs concurrently with the Newton iteration (warp specialisation, two named barriers).
 // MODE_DROOP runs the paper's droop-control baseline (a relaxed loop of power flows) inside the same kernel; the host
 // path can hand the kernel pinned host memory for actions / results (mapdn_step_host_pinned: no staging copies).
+// Handles with observation history (mapdn_set_history) step with the HIST instantiations: the epilogue also records the
+// newest frame in a per-env ring in HBM and can write the stacked rows of the last `history` frames (get_obs :303-315).
 //
 // The linear solve works on the forest of PQ buses (the slack bus is not an unknown), each tree
 // re-rooted at its centre so that the leaf->root elimination has half the depth of the feeder.
@@ -757,12 +759,46 @@ __device__ __forceinline__ double clip_q(double a, double pv, double smax) {
   return sqrt(smax * smax - pv * pv) * a;
 }
 
+// Stacked observation row of one env (reference get_obs :303-315): agent a's block k (oldest first) is frame
+// f - (history - 1) + k; a frame with a negative index (before the episode start) is zero, the others come from the ring.
+// newest(i) gives entry i of frame f when the caller holds it elsewhere (the step kernel: its shared-memory slab). Lanes
+// lane, lane + nlanes, ... store consecutive 16-byte pieces (even obs_dim), else single entries.
+template <class Newest>
+__device__ __forceinline__ void write_stacked_row(const Params& p, int env, int f, int lane, int nlanes, Newest newest) {
+  const int od = p.obs_dim, H = p.history, tot = p.n_sgen * od, blk = H * od;
+  const double* ring = p.hist + static_cast<size_t>(env) * H * tot;
+  double* o = p.obs_stacked + static_cast<size_t>(env) * p.n_sgen * blk;
+  auto entry = [&](int e, double* v, int n) {        // n consecutive entries from e (inside one frame block)
+    const int a = e / blk, r = e - a * blk, k = r / od, j = r - k * od;
+    const int fk = f - (H - 1) + k, i = a * od + j;
+    for (int u = 0; u < n; ++u) v[u] = 0.0;
+    if (fk < 0) return;
+    if (k == H - 1) { for (int u = 0; u < n; ++u) v[u] = newest(i + u); return; }
+    const double* src = ring + static_cast<size_t>(fk % H) * tot + i;
+    if (n == 2) { const double2 w = *reinterpret_cast<const double2*>(src); v[0] = w.x; v[1] = w.y; }
+    else v[0] = *src;
+  };
+  const int row = p.n_sgen * blk;
+  if ((od & 1) == 0 && (reinterpret_cast<uintptr_t>(p.obs_stacked) & 15) == 0) {
+    for (int c = lane; c < row / 2; c += nlanes) {
+      double v[2];
+      entry(2 * c, v, 2);
+      *reinterpret_cast<double2*>(o + 2 * c) = make_double2(v[0], v[1]);
+    }
+  } else {
+    for (int e = lane; e < row; e += nlanes) { double v[1]; entry(e, v, 1); o[e] = v[0]; }
+  }
+}
+
 // RECORD (MODE_STEP only): the epilogue also writes the env's tester record row (see Params::record) from the values it
-// already holds. A template flag, so the instantiations without it are the same code as before it existed.
-template <int G, int MODE, bool DENSE = false, bool RECORD = false>
+// already holds. HIST (MODE_STEP only, handles with history): the epilogue also writes the env's newest observation frame
+// into its slot of the ring and, when Params::obs_stacked is set, the stacked row. Template flags, so the instantiations
+// without them are the same code as before they existed.
+template <int G, int MODE, bool DENSE = false, bool RECORD = false, bool HIST = false>
 __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_constant__ Params p) {
   static_assert(!DENSE || G == 32, "the dense fallback uses one warp per env");
   static_assert(!RECORD || MODE == MODE_STEP, "records are written by the step kernel");
+  static_assert(!HIST || MODE == MODE_STEP, "the frame ring is written by the step kernel (resets: reset_frame_kernel)");
   static_assert(G == 4 || G == 8 || G == 16 || G == 32 || G == 64 || G == 128, "unsupported group size");
 #ifdef MAPDN_HOST_EMU
   unsigned char* const smem_raw = emu::dyn_smem();
@@ -1360,6 +1396,22 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
       };
       if (h.in_blob && !compact) gather(reinterpret_cast<const uint16_t*>(smem_raw + hl.obs_off), std::false_type{});
       else gather(compact ? p.obs_compact_prog : p.obs_off, std::true_type{});
+    }
+    if constexpr (HIST) {
+      // frame f = steps - 1 of this step into its ring slot, through the padded program whatever layout (compact, fp32,
+      // none) the caller's observations take; then the stacked row, whose newest frame comes straight from the slab
+      if (valid) {
+        const int f = steps_old, tot = ng * p.obs_dim;
+        const uint16_t* prog = h.in_blob ? reinterpret_cast<const uint16_t*>(smem_raw + hl.obs_off) : p.obs_off;
+        double* fr = p.hist + (static_cast<size_t>(env) * p.history + f % p.history) * tot;
+        if ((tot & 1) == 0) {
+          for (int c = gl; c < tot / 2; c += G)
+            *reinterpret_cast<double2*>(fr + 2 * c) = make_double2(s.base[prog[2 * c]], s.base[prog[2 * c + 1]]);
+        } else {
+          for (int i = gl; i < tot; i += G) fr[i] = s.base[prog[i]];
+        }
+        if (p.obs_stacked != nullptr) write_stacked_row(p, env, f, gl, G, [&](int i) { return s.base[prog[i]]; });
+      }
     }
     if (MODE == MODE_RESET && p.state != nullptr) {
       // get_state (:213-230): [P_bus | Q_bus | pv | q | vm | va(deg)] restricted to state_space (cold program)

@@ -135,6 +135,13 @@ struct Params {
   // [pv n_sgen | q n_sgen | P_bus n_bus | Q_bus n_bus | vm n_bus | line loss n_line]
   double* record;
   long long record_stride;
+  // observation history (mapdn_set_history, history > 1): frame ring [B][history][n_sgen * obs_dim] (the padded get_obs
+  // layout). Frame f of an env counts the frames since its last reset (f = steps - 1) and lives in slot f mod history.
+  double* hist;
+  int history;            // 1: no ring
+  // MODE_STEP of a handle with history (or NULL): stacked rows [B, n_sgen, history * obs_dim], oldest frame first, zero
+  // frames before the episode start (reference get_obs :303-315)
+  double* obs_stacked;
 };
 
 // cold obs program entry: kind in the top 4 bits, node / sgen index in the low 28

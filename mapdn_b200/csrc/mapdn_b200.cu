@@ -114,12 +114,8 @@ __global__ void i64_to_double_kernel(long long n, const long long* __restrict__ 
   if (i < n) out[i] = static_cast<double>(in[i]);
 }
 
-// get_obs() from the state in HBM (reference :232-316), driven by the precomputed obs program
-__global__ void get_obs_kernel(const __grid_constant__ Params p) {
-  const int tot = p.n_sgen * p.obs_dim;
-  const long long gid = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
-  if (gid >= static_cast<long long>(p.nb) * tot) return;
-  const int env = static_cast<int>(gid / tot), idx = static_cast<int>(gid - static_cast<long long>(env) * tot);
+// entry idx of get_obs() of env `env` from the state in HBM (reference :232-316), driven by the precomputed obs program
+__device__ __forceinline__ double obs_entry(const Params& p, int env, int idx) {
   const size_t eN = static_cast<size_t>(env) * p.n_bus, eG = static_cast<size_t>(env) * p.n_sgen;
   const unsigned src = __ldg(p.obs_src + idx);   // cold copy of the obs program (kind | node)
   const int kind = static_cast<int>(src >> 28), ix = static_cast<int>(src & 0x0FFFFFFFu);
@@ -136,7 +132,40 @@ __global__ void get_obs_kernel(const __grid_constant__ Params p) {
   else if (kind == OBS_QSG) v = p.cur_q[eG + ix];
   else if (kind == OBS_VM) v = p.res_vm[eN + bus(ix)];
   else if (kind == OBS_VA) v = p.res_va[eN + bus(ix)];
-  p.obs[gid] = v;
+  return v;
+}
+
+__global__ void get_obs_kernel(const __grid_constant__ Params p) {
+  const int tot = p.n_sgen * p.obs_dim;
+  const long long gid = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  if (gid >= static_cast<long long>(p.nb) * tot) return;
+  const int env = static_cast<int>(gid / tot), idx = static_cast<int>(gid - static_cast<long long>(env) * tot);
+  p.obs[gid] = obs_entry(p, env, idx);
+}
+
+// history > 1, after a reset launch: frame 0 of the new episode of every reset env (mask) into ring slot 0
+__global__ void reset_frame_kernel(const __grid_constant__ Params p) {
+  const int tot = p.n_sgen * p.obs_dim;
+  const long long gid = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  if (gid >= static_cast<long long>(p.nb) * tot) return;
+  const int env = static_cast<int>(gid / tot), idx = static_cast<int>(gid - static_cast<long long>(env) * tot);
+  if (p.mask != nullptr && !p.mask[env]) return;
+  p.hist[static_cast<size_t>(env) * p.history * tot + idx] = obs_entry(p, env, idx);
+}
+
+// mapdn_get_obs_stacked: the stacked rows from the ring and the step counters - the rule the step kernel applies in its
+// epilogue, one 16-byte piece (even obs_dim) or one entry per thread
+__global__ void obs_stacked_kernel(const __grid_constant__ Params p) {
+  const int per = (p.obs_dim & 1) == 0 ? 2 : 1;
+  const int row = p.n_sgen * p.history * p.obs_dim / per;                  // pieces per env
+  const long long gid = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  if (gid >= static_cast<long long>(p.nb) * row) return;
+  const int env = static_cast<int>(gid / row), c = static_cast<int>(gid - static_cast<long long>(env) * row);
+  const double* ring = p.hist + static_cast<size_t>(env) * p.history * p.n_sgen * p.obs_dim;
+  // the newest frame is in the ring too: write_stacked_row reads it there, restricted to this thread's piece
+  write_stacked_row(p, env, p.steps[env] - 1, c, row, [&](int i) {
+    return ring[static_cast<size_t>((p.steps[env] - 1) % p.history) * p.n_sgen * p.obs_dim + i];
+  });
 }
 
 // get_state() (reference :213-230): [P_bus | Q_bus | pv | q | vm | va(deg)] restricted to state_space
@@ -187,6 +216,7 @@ struct mapdn_env {
   std::vector<void*> allocs;           // everything cudaMalloc'ed
   int G = 8, threads = 128, epb = 16, smem = 0, max_blocks = 0, helper_threads = 32;
   int max_blocks_record = 0;           // persistent grid of the MODE_STEP instantiation with tester records
+  int max_blocks_hist = 0, max_blocks_hist_record = 0;   // the same for the HIST instantiations (observation history)
   bool dense = false;                  // meshed net: dense-LU fallback solver
   long long launches = 0;
   // Ybus pieces kept for the test hook
@@ -234,25 +264,28 @@ using KernelFn = void (*)(const Params);
 constexpr int kHelperPairsPerWarp = 256;   // Box-Muller pairs of a CTA round per helper warp
 
 template <int G, bool DENSE>
-KernelFn kernel_for_mode(int mode, bool record) {
+KernelFn kernel_for_mode(int mode, bool record, bool hist) {
   switch (mode) {
     case MODE_SOLVE: return env_kernel<G, MODE_SOLVE, DENSE>;
-    case MODE_STEP: return record ? env_kernel<G, MODE_STEP, DENSE, true> : env_kernel<G, MODE_STEP, DENSE>;
+    case MODE_STEP:
+      if (hist) return record ? env_kernel<G, MODE_STEP, DENSE, true, true> : env_kernel<G, MODE_STEP, DENSE, false, true>;
+      return record ? env_kernel<G, MODE_STEP, DENSE, true> : env_kernel<G, MODE_STEP, DENSE>;
     case MODE_DROOP: return env_kernel<G, MODE_DROOP, DENSE>;
     default: return env_kernel<G, MODE_RESET, DENSE>;
   }
 }
 
-// record: the MODE_STEP instantiation that also writes the tester record rows (mapdn_step_record)
-KernelFn kernel_for(int G, int mode, bool dense = false, bool record = false) {
-  if (dense) return kernel_for_mode<32, true>(mode, record);
+// record: the MODE_STEP instantiation that also writes the tester record rows (mapdn_step_record); hist: the one that
+// also records observation frames (handles with history)
+KernelFn kernel_for(int G, int mode, bool dense = false, bool record = false, bool hist = false) {
+  if (dense) return kernel_for_mode<32, true>(mode, record, hist);
   switch (G) {
-    case 4: return kernel_for_mode<4, false>(mode, record);
-    case 8: return kernel_for_mode<8, false>(mode, record);
-    case 16: return kernel_for_mode<16, false>(mode, record);
-    case 64: return kernel_for_mode<64, false>(mode, record);
-    case 128: return kernel_for_mode<128, false>(mode, record);
-    default: return kernel_for_mode<32, false>(mode, record);
+    case 4: return kernel_for_mode<4, false>(mode, record, hist);
+    case 8: return kernel_for_mode<8, false>(mode, record, hist);
+    case 16: return kernel_for_mode<16, false>(mode, record, hist);
+    case 64: return kernel_for_mode<64, false>(mode, record, hist);
+    case 128: return kernel_for_mode<128, false>(mode, record, hist);
+    default: return kernel_for_mode<32, false>(mode, record, hist);
   }
 }
 
@@ -277,9 +310,12 @@ int env_stride2_for(int npq, int ng, int nl, int G, bool stage_rec) {
 
 mapdn_status launch_env_kernel(mapdn_env* e, int mode, Params& p, cudaStream_t st) {
   const bool record = mode == MODE_STEP && p.record != nullptr;
-  KernelFn fn = kernel_for(e->G, mode, e->dense, record);
+  const bool hist = mode == MODE_STEP && p.history > 1;      // every step of a handle with history records its frame
+  KernelFn fn = kernel_for(e->G, mode, e->dense, record, hist);
   const int needed = (p.nb + e->epb - 1) / e->epb;
-  int grid = std::min(needed, std::max(1, record ? e->max_blocks_record : e->max_blocks));
+  const int max_blocks = hist ? (record ? e->max_blocks_hist_record : e->max_blocks_hist)
+                              : (record ? e->max_blocks_record : e->max_blocks);
+  int grid = std::min(needed, std::max(1, max_blocks));
   const int rounds = (needed + grid - 1) / grid;
   grid = (needed + rounds - 1) / rounds;       // balance the persistent loop
 #ifdef MAPDN_PROFILE
@@ -321,7 +357,8 @@ constexpr auto nothing = [](cudaStream_t) { return MAPDN_OK; };   // before / af
 template <class Before, class After>
 mapdn_status step(mapdn_env* e, const double* actions, int32_t add_noise, double* reward, uint8_t* term, double* info,
                   void* obs, bool obs_f32, void* stream, Before before, After after, int obs_skip_off = -1,
-                  int obs_compact_len = 0, double* record = nullptr, int64_t record_stride = 0) {
+                  int obs_compact_len = 0, double* record = nullptr, int64_t record_stride = 0,
+                  double* obs_stacked = nullptr) {
   if (!e->base.prof_pv) return fail(MAPDN_ERR_INVALID, "handle was created without a profile store");
   MAPDN_ON_DEVICE(e->device);
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -331,6 +368,7 @@ mapdn_status step(mapdn_env* e, const double* actions, int32_t add_noise, double
   p.actions = actions; p.add_noise = add_noise; p.reward = reward; p.term = term; p.info = info;
   p.obs = obs_f32 ? nullptr : static_cast<double*>(obs); p.obs32 = obs_f32 ? static_cast<float*>(obs) : nullptr;
   p.obs_skip_off = obs_skip_off; p.obs_compact_len = obs_compact_len; p.record = record; p.record_stride = record_stride;
+  p.obs_stacked = obs_stacked;
   s = launch_env_kernel(e, MODE_STEP, p, st);
   return s != MAPDN_OK ? s : after(st);
 }
@@ -1082,8 +1120,8 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
     e->helper_threads = 32 * std::min(4, std::max(1, (epb * n_pair + kHelperPairsPerWarp - 1) / kHelperPairsPerWarp));
   }
   if (const char* ov = getenv("MAPDN_HELPERS")) e->helper_threads = 32 * std::min(4, std::max(1, atoi(ov)));   // tuning override
-  for (int mode = 0; mode < 5; ++mode) {      // 4: the MODE_STEP instantiation with tester records
-    KernelFn fn = (mode < 4) ? kernel_for(G, mode, meshed) : kernel_for(G, MODE_STEP, meshed, true);
+  for (int mode = 0; mode < 7; ++mode) {      // 4: MODE_STEP with tester records; 5, 6: with history, without / with records
+    KernelFn fn = (mode < 4) ? kernel_for(G, mode, meshed) : kernel_for(G, MODE_STEP, meshed, mode != 5, mode > 4);
     // the attribute belongs to the function, not to the handle: always allow the device maximum, so that creating a
     // second handle with a smaller footprint cannot break the launches of the first
     cudaFuncAttributes fa{};
@@ -1101,6 +1139,10 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
     // the record instantiation holds more registers: its persistent grid is sized by its own occupancy (never larger)
     TRY_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel_for(G, MODE_STEP, meshed, true), e->threads + e->helper_threads, e->smem));
     e->max_blocks_record = std::min(e->max_blocks, std::max(1, per_sm) * dp.multiProcessorCount);
+    TRY_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel_for(G, MODE_STEP, meshed, false, true), e->threads + e->helper_threads, e->smem));
+    e->max_blocks_hist = std::min(e->max_blocks, std::max(1, per_sm) * dp.multiProcessorCount);
+    TRY_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel_for(G, MODE_STEP, meshed, true, true), e->threads + e->helper_threads, e->smem));
+    e->max_blocks_hist_record = std::min(e->max_blocks, std::max(1, per_sm) * dp.multiProcessorCount);
   }
 
   // ---- 6. upload + env state ----
@@ -1114,6 +1156,7 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
   P.helper_off = hl.bytes + e->epb * stride2 * 16;
   P.stage_in_records = stage_rec ? 1 : 0;
   P.obs_skip_off = -1;
+  P.history = 1;
   e->obs_zero_off = 2 * (npq * kNodeArrays2 + A_UP);
   TRY(dev_upload(e, obs_compact, &P.obs_compact_prog));
   P.obs_compact_len = 0;
@@ -1290,7 +1333,29 @@ mapdn_status mapdn_reset(mapdn_env* e, const int32_t* start_dhi_dev, const uint8
   Params p = e->base;
   p.start_dhi = start_dhi_dev; p.mask = mask_dev; p.add_noise = add_noise; p.obs = obs_dev; p.state = state_dev;
   p.reset_ok = converged_dev;
-  return launch_env_kernel(e, MODE_RESET, p, static_cast<cudaStream_t>(stream));
+  mapdn_status s = launch_env_kernel(e, MODE_RESET, p, static_cast<cudaStream_t>(stream));
+  if (s != MAPDN_OK || p.history <= 1) return s;
+  // frame 0 of the new episodes into ring slot 0 (the reset kernel itself has no history instantiation)
+  return gather(e, reset_frame_kernel, static_cast<long long>(p.nb) * p.n_sgen * p.obs_dim, stream, p);
+}
+
+mapdn_status mapdn_set_history(mapdn_env* e, int32_t history) {
+  if (!e) return fail(MAPDN_ERR_INVALID, "null handle");
+  if (history < 1) return fail(MAPDN_ERR_INVALID, "history must be >= 1");
+  MAPDN_ON_DEVICE(e->device);
+  Params& P = e->base;
+  if (P.hist) {                 // cudaFree waits for the launches still reading the ring
+    MAPDN_CUDA(cudaFree(P.hist));
+    e->allocs.erase(std::find(e->allocs.begin(), e->allocs.end(), static_cast<void*>(P.hist)));
+    P.hist = nullptr;
+  }
+  P.history = 1;
+  if (history == 1) return MAPDN_OK;
+  const mapdn_status s = dev_alloc(e, static_cast<size_t>(P.nb) * history * P.n_sgen * P.obs_dim, &P.hist);
+  if (s != MAPDN_OK) return s;
+  MAPDN_CUDA(cudaDeviceSynchronize());     // the zero fill ran on the legacy default stream: order it before any launch
+  P.history = history;
+  return MAPDN_OK;
 }
 
 mapdn_status mapdn_step(mapdn_env* e, const double* actions_dev, int32_t add_noise, double* reward_dev,
@@ -1328,6 +1393,27 @@ mapdn_status mapdn_step_record(mapdn_env* e, const double* actions_dev, int32_t 
   };
   return step(e, actions_dev, add_noise, reward_dev, terminated_dev, info_dev, obs_dev, false, stream, check_stride, nothing,
               -1, 0, record_dev, record_stride);
+}
+
+static int stacked_row_len(const mapdn_env* e) { return e->base.history * e->dims.n_sgen * e->dims.obs_dim; }
+
+mapdn_status mapdn_step_stacked(mapdn_env* e, const double* actions_dev, int32_t add_noise, double* reward_dev,
+                                uint8_t* terminated_dev, double* info_dev, double* obs_dev, double* obs_stacked_dev,
+                                double* record_dev, int64_t record_stride, void* stream) {
+  if (!e || !actions_dev || !reward_dev || !terminated_dev) return fail(MAPDN_ERR_INVALID, "null argument");
+  if (e->base.history <= 1) return fail(MAPDN_ERR_INVALID, "handle has no observation history (mapdn_set_history)");
+  if (record_dev && record_stride < record_row_len(e)) return fail(MAPDN_ERR_INVALID, "record_stride shorter than a record row");
+  return step(e, actions_dev, add_noise, reward_dev, terminated_dev, info_dev, obs_dev, false, stream, nothing, nothing,
+              -1, 0, record_dev, record_stride, obs_stacked_dev);
+}
+
+mapdn_status mapdn_get_obs_stacked(mapdn_env* e, double* obs_stacked_dev, void* stream) {
+  if (!e || !obs_stacked_dev) return fail(MAPDN_ERR_INVALID, "null argument");
+  if (e->base.history <= 1) return fail(MAPDN_ERR_INVALID, "handle has no observation history (mapdn_set_history)");
+  Params p = e->base;
+  p.obs_stacked = obs_stacked_dev;
+  const long long pieces = static_cast<long long>(p.nb) * stacked_row_len(e) / ((p.obs_dim & 1) == 0 ? 2 : 1);
+  return gather(e, obs_stacked_kernel, pieces, stream, p);
 }
 
 mapdn_status mapdn_step_host(mapdn_env* e, const double* actions_host, int32_t add_noise, double* reward_host,

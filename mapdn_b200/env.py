@@ -103,7 +103,13 @@ class BatchedVoltageControl:
             self.terminated = torch.zeros(B, dtype=torch.uint8, device=self.device)
             self.info = torch.zeros(B, len(INFO_KEYS), dtype=f64, device=self.device)
             self.reset_ok = torch.ones(B, dtype=torch.uint8, device=self.device)
-        self._hist = None       # [B, history, n_agents, obs_dim] ring of the last observations (history > 1)
+        # history > 1 (reference :303-315): the step kernel keeps a ring of the last frames and writes the stacked rows
+        # [B, n_agents, history * obs_dim] here; a learner is sized with stacked_obs_size
+        self.stacked_obs_size = self.history * self.obs_size
+        self.obs_stacked = self.obs
+        if self.history > 1:
+            _capi.check(L.mapdn_set_history(h, self.history))
+            self.obs_stacked = torch.zeros(B, d.n_agents, self.stacked_obs_size, dtype=f64, device=self.device)
         self._host = None
         # raw pointers of the internal buffers (ctypes converts plain ints for c_void_p parameters): keeps the
         # per-step Python overhead of the hot call small
@@ -171,18 +177,14 @@ class BatchedVoltageControl:
         if mask is not None and want_state:   # state of the untouched envs
             _capi.check(self._L.mapdn_get_state(self._h, _ptr(self.state), self._stream()))
         if self.history > 1:
-            if self._hist is None or mask is None:
-                self._hist = torch.zeros(self.batch, self.history, self.n_agents, self.obs_size, dtype=torch.float64,
-                                         device=self.device)
-            else:
-                self._hist[mask.bool()] = 0.0
-            self._hist[:, -1] = self.obs
+            _capi.check(self._L.mapdn_get_obs_stacked(self._h, _ptr(self.obs_stacked), self._stream()))
         return self.obs, self.state
 
     def step(self, actions: torch.Tensor, add_noise: bool = True, want_obs: bool = True, want_info: bool = True,
              record: Optional[torch.Tensor] = None):
         """One transition of every env. Returns (reward ``[B]``, terminated ``[B]`` uint8,
-        info ``[B,11]`` in INFO_KEYS order); the new observations are in ``self.obs``.
+        info ``[B,11]`` in INFO_KEYS order); the new observations are in ``self.obs`` and, with ``history > 1``, the
+        stacked rows in ``self.obs_stacked`` (the same launch; ``want_obs=False`` skips both, the frame is still recorded).
 
         ``record``: an fp64 ``[B, record_len]`` view with unit column stride and any row stride (row ``t`` of a
         ``[B, T + 1, record_len]`` tensor): the same kernel launch also writes every env's tester record after the step
@@ -191,7 +193,13 @@ class BatchedVoltageControl:
                 or not actions.is_contiguous()):
             self._chk(actions, self._act_shape, name="actions")
         stream = torch.cuda.current_stream(self.device).cuda_stream
-        if record is not None:
+        if self.history > 1:
+            st = self._L.mapdn_step_stacked(self._h, actions.data_ptr(), int(add_noise), self._p_reward, self._p_term,
+                                            self._p_info if want_info else None, self._p_obs if want_obs else None,
+                                            self.obs_stacked.data_ptr() if want_obs else None,
+                                            None if record is None else record.data_ptr(),
+                                            0 if record is None else self._record_stride(record), stream)
+        elif record is not None:
             st = self._L.mapdn_step_record(self._h, actions.data_ptr(), int(add_noise), self._p_reward, self._p_term,
                                            self._p_info if want_info else None, self._p_obs if want_obs else None,
                                            record.data_ptr(), self._record_stride(record), stream)
@@ -200,9 +208,6 @@ class BatchedVoltageControl:
                                     self._p_info if want_info else None, self._p_obs if want_obs else None, stream)
         if st:
             _capi.check(st)
-        if self.history > 1 and want_obs and self._hist is not None:
-            self._hist = torch.roll(self._hist, -1, dims=1)
-            self._hist[:, -1] = self.obs
         return self.reward, self.terminated, self.info
 
     # host-buffer path (what a CPU-side caller such as the reference trainer pays end to end)
@@ -239,8 +244,6 @@ class BatchedVoltageControl:
         f32 = np.dtype(obs_dtype) == np.float32
         stream = torch.cuda.current_stream(self.device).cuda_stream
         if layout == "compact":
-            if self.history > 1:
-                raise NotImplementedError("compact host rows carry one frame (history = 1)")
             row = self.obs_row_len
             key = "obs_c32" if f32 else "obs_c"
             if key not in hb:
@@ -308,10 +311,13 @@ class BatchedVoltageControl:
 
     def get_obs_stacked(self) -> torch.Tensor:
         """``history`` stacked observations ``[B, n_agents, history * obs_dim]``, oldest frame first and zero frames
-        before the episode start (reference :303-315; one frame per reset / step, not per ``get_obs`` call)."""
-        if self.history <= 1 or self._hist is None:
+        before the episode start (reference :303-315; one frame per reset / step, not per ``get_obs`` call), in a new
+        tensor gathered from the device's frame ring: current after every reset and step, host-path steps included."""
+        if self.history <= 1:
             return self.obs
-        return self._hist.permute(0, 2, 1, 3).reshape(self.batch, self.n_agents, self.history * self.obs_size)
+        out = torch.empty_like(self.obs_stacked)
+        _capi.check(self._L.mapdn_get_obs_stacked(self._h, _ptr(out), self._stream()))
+        return out
 
     # ---- getters ------------------------------------------------------------------------------
     def get_obs(self) -> torch.Tensor:

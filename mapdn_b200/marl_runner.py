@@ -142,6 +142,12 @@ class DeviceTransitionBuffer:
         return DeviceBatch(out)
 
 
+def learner_obs(env) -> torch.Tensor:
+    """What the learner consumes after a reset or step: the stacked frames ``[B, n_agents, history * obs_dim]`` of an env
+    with observation history (``history > 1``, reference :303-315), else the observations ``env.obs``."""
+    return env.obs_stacked if getattr(env, "history", 1) > 1 else env.obs
+
+
 class BatchedMarlRunner:
     """``Model.train_process`` / ``Model.evaluation`` over B lock-step envs (see module docstring).
 
@@ -166,8 +172,8 @@ class BatchedMarlRunner:
     def train_process(self, stat: dict) -> dict:
         env, net, args = self.env, self.net, self.args
         B = env.batch
-        obs, _ = env.reset()
-        state = obs.to(torch.float32).clone()
+        env.reset()
+        state = learner_obs(env).to(torch.float32).clone()
         last_hid = self._init_hidden()
         info_sum = torch.zeros(len(INFO_KEYS), dtype=torch.float64, device=env.device)
         reward_sum = torch.zeros((), dtype=torch.float64, device=env.device)
@@ -178,7 +184,7 @@ class BatchedMarlRunner:
                                                                      last_hid=last_hid)
             value = net.value(state, action_pol)
             reward, done, info = env.step(self._translate(action))
-            next_state = env.obs.to(torch.float32).clone()
+            next_state = learner_obs(env).to(torch.float32).clone()
             _, next_action_pol, _, _, _ = net.get_actions(next_state, status="train", exploration=True,
                                                           actions_avail=self._avail, target=False, last_hid=hid)
             next_value = net.value(next_state, next_action_pol)
@@ -199,7 +205,7 @@ class BatchedMarlRunner:
             # envs that ended early (divergence) start a new episode right away; the others carry on
             env.reset(mask=done, want_state=False)
             keep = (1.0 - done_f)[:, :, None]
-            state = torch.where(done.bool()[:, None, None], env.obs.to(torch.float32), next_state)
+            state = torch.where(done.bool()[:, None, None], learner_obs(env).to(torch.float32), next_state)
             last_hid = hid.detach() * keep
         self.episodes += B
         denom = float(n_steps * B)
@@ -217,8 +223,8 @@ class BatchedMarlRunner:
         rounds = max(1, -(-int(num_eval_episodes or args.num_eval_episodes) // B))
         tot = torch.zeros(len(INFO_KEYS) + 1, dtype=torch.float64, device=env.device)
         for _ in range(rounds):
-            obs, _ = env.reset()
-            state = obs.to(torch.float32).clone()
+            env.reset()
+            state = learner_obs(env).to(torch.float32).clone()
             last_hid = self._init_hidden()
             alive = torch.ones(B, dtype=torch.float64, device=env.device)
             acc = torch.zeros(B, len(INFO_KEYS) + 1, dtype=torch.float64, device=env.device)
@@ -230,7 +236,7 @@ class BatchedMarlRunner:
                 acc += alive[:, None] * torch.cat([reward[:, None], info], dim=1)
                 cnt += alive
                 alive = alive * (1.0 - done.to(torch.float64))
-                state, last_hid = env.obs.to(torch.float32).clone(), hid
+                state, last_hid = learner_obs(env).to(torch.float32).clone(), hid
             tot += (acc / cnt[:, None]).mean(dim=0)
         tot = (tot / rounds).tolist()
         stat["mean_test_reward"] = tot[0]
@@ -277,7 +283,7 @@ class BatchedPolicyTester:
             buf = records[c0:c0 + n] if n == B else torch.full((B, T + 1, R), nan, dtype=torch.float64, device=dev)
             env.reset(start, add_noise=False, check=True)                                     # tester.py:21
             env.record(buf[:, 0])                                                             # :34-39
-            state = env.obs.to(torch.float32).clone()
+            state = learner_obs(env).to(torch.float32).clone()
             last_hid = self._runner._init_hidden()
             alive = torch.ones(B, dtype=torch.bool, device=dev)
             length = torch.ones(B, dtype=torch.int64, device=dev)
@@ -286,7 +292,7 @@ class BatchedPolicyTester:
                 _, done, _ = env.step(actions, add_noise=False, record=buf[:, t + 1])           # :48-55
                 length += alive
                 alive &= done == 0                                                            # :49, :61
-                state, last_hid = env.obs.to(torch.float32).clone(), hid
+                state, last_hid = learner_obs(env).to(torch.float32).clone(), hid
             rows = torch.arange(T + 1, device=dev)[None, :, None]
             buf.masked_fill_(rows >= length[:, None, None], nan)
             if n < B:
@@ -319,7 +325,7 @@ class BatchedPolicyTester:
         for r0 in range(0, num_episodes, B):
             vals.zero_(); mask.zero_()
             env.reset(check=True)                                                             # tester.py:69
-            state = env.obs.to(torch.float32).clone()
+            state = learner_obs(env).to(torch.float32).clone()
             last_hid = self._runner._init_hidden()
             alive = torch.arange(B, device=dev) < num_episodes - r0                           # spare envs of the last round
             for t in range(T):
@@ -328,7 +334,7 @@ class BatchedPolicyTester:
                 vals[t] = info
                 mask[t] = alive.to(torch.float64)                                             # :84-88
                 alive &= done == 0                                                            # :82, :93
-                state, last_hid = env.obs.to(torch.float32).clone(), hid
+                state, last_hid = learner_obs(env).to(torch.float32).clone(), hid
             # this round's pooled statistics (two-pass), merged into the running ones (Chan et al.)
             nr = mask.sum()
             mr = (vals * mask[..., None]).sum(dim=(0, 1)) / nr
