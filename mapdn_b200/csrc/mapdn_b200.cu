@@ -8,6 +8,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <new>
 #include <string>
 #include <utility>
@@ -38,6 +39,11 @@ static mapdn_status fail(mapdn_status st, const std::string& msg) {
     cudaError_t _e = (expr);                                                                    \
     if (_e != cudaSuccess)                                                                      \
       return fail(MAPDN_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e));          \
+  } while (0)
+#define MAPDN_TRY(expr)                                                                         \
+  do {                                                                                          \
+    const mapdn_status _s = (expr);                                                             \
+    if (_s != MAPDN_OK) return _s;                                                              \
   } while (0)
 
 // Every entry point runs on the handle's device and leaves the calling thread's current device as it found it
@@ -214,9 +220,8 @@ struct mapdn_env {
   mapdn_dims dims{};
   Params base{};                       // static + state pointers; io fields filled per call
   std::vector<void*> allocs;           // everything cudaMalloc'ed
-  int G = 8, threads = 128, epb = 16, smem = 0, max_blocks = 0, helper_threads = 32;
-  int max_blocks_record = 0;           // persistent grid of the MODE_STEP instantiation with tester records
-  int max_blocks_hist = 0, max_blocks_hist_record = 0;   // the same for the HIST instantiations (observation history)
+  int G = 8, threads = 128, epb = 16, smem = 0, helper_threads = 32;
+  int max_blocks_step[2][2] = {};      // persistent grid of the MODE_STEP instantiations [observation history][tester records]
   bool dense = false;                  // meshed net: dense-LU fallback solver
   long long launches = 0;
   // Ybus pieces kept for the test hook
@@ -313,9 +318,7 @@ mapdn_status launch_env_kernel(mapdn_env* e, int mode, Params& p, cudaStream_t s
   const bool hist = mode == MODE_STEP && p.history > 1;      // every step of a handle with history records its frame
   KernelFn fn = kernel_for(e->G, mode, e->dense, record, hist);
   const int needed = (p.nb + e->epb - 1) / e->epb;
-  const int max_blocks = hist ? (record ? e->max_blocks_hist_record : e->max_blocks_hist)
-                              : (record ? e->max_blocks_record : e->max_blocks);
-  int grid = std::min(needed, std::max(1, max_blocks));
+  int grid = std::min(needed, std::max(1, e->max_blocks_step[hist][record]));
   const int rounds = (needed + grid - 1) / grid;
   grid = (needed + rounds - 1) / rounds;       // balance the persistent loop
 #ifdef MAPDN_PROFILE
@@ -424,25 +427,12 @@ mapdn_status gather(mapdn_env* e, Kernel kernel, long long n, void* stream, Args
   return MAPDN_OK;
 }
 
-}  // namespace
-
-extern "C" {
-
-int32_t mapdn_abi_version(void) { return MAPDN_ABI_VERSION; }
-const char* mapdn_last_error(void) { return g_last_error.c_str(); }
-
-mapdn_status mapdn_destroy(mapdn_env* e) {
-  if (!e) return MAPDN_OK;
-  DeviceGuard guard(e->device);
-  for (void* d : e->allocs) cudaFree(d);
-  delete e;
-  return MAPDN_OK;
-}
-
-mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* prof, const mapdn_cfg* cfg,
-                          int32_t device, mapdn_env** out) {
-  if (!net || !cfg || !out) return fail(MAPDN_ERR_INVALID, "null argument");
-  *out = nullptr;
+// ------------------------------------------------------------------------------------------------
+// mapdn_create, stage by stage. Between the Ybus assembly and the kernel attributes every stage is host arithmetic on
+// plain structs: no CUDA call, no handle. Each takes what it reads by const reference, so the order of the calls in
+// mapdn_create is the only order dependency.
+// ------------------------------------------------------------------------------------------------
+mapdn_status validate_create_args(const mapdn_net_desc* net, const mapdn_profile_desc* prof, const mapdn_cfg* cfg) {
   const int n = net->n_bus, nbr = net->n_branch, nl = net->n_load, ng = net->n_sgen;
   if (n < 2 || n > 65000) return fail(MAPDN_ERR_INVALID, "n_bus must be in [2, 65000]");
   if (nbr < 1 || nl < 0 || ng < 1) return fail(MAPDN_ERR_INVALID, "need >=1 branch and >=1 sgen");
@@ -469,66 +459,94 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
         !prof->load_q_std || !prof->s_max || prof->n_rows < 2 || prof->steps_per_hour < 1)
       return fail(MAPDN_ERR_INVALID, "incomplete profile description");
   }
-  MAPDN_ON_DEVICE(device);
-  mapdn_env* e = new (std::nothrow) mapdn_env();
-  if (!e) return fail(MAPDN_ERR_NOMEM, "out of host memory");
-  e->device = device;
-  e->cfg = *cfg;
-  mapdn_status st = MAPDN_OK;
-  auto bail = [&](mapdn_status s) { mapdn_destroy(e); return s; };
-#define TRY(expr) do { st = (expr); if (st != MAPDN_OK) return bail(st); } while (0)
-#define TRY_CUDA(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) { \
-      fail(MAPDN_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e)); return bail(MAPDN_ERR_CUDA); } } while (0)
+  return MAPDN_OK;
+}
 
-  // ---- 1. Ybus on the device ----
-  std::vector<double> br_r(net->br_r, net->br_r + nbr), br_x(net->br_x, net->br_x + nbr);
-  std::vector<double> br_b = vec_or(net->br_b, nbr, 0.0), br_g = vec_or(net->br_g, nbr, 0.0);
-  std::vector<double> br_tap = vec_or(net->br_tap, nbr, 1.0), br_sh = vec_or(net->br_shift_deg, nbr, 0.0);
-  std::vector<unsigned char> br_st = vec_or<unsigned char>(net->br_status, nbr, 1);
-  std::vector<unsigned char> br_line = vec_or<unsigned char>(net->br_is_line, nbr, 1);
-  std::vector<double> gs = vec_or(net->bus_gs_mw, n, 0.0), bs = vec_or(net->bus_bs_mvar, n, 0.0);
-  e->br_from.assign(net->br_from, net->br_from + nbr);
-  e->br_to.assign(net->br_to, net->br_to + nbr);
+// The branch and shunt arrays with the optional ones filled in, and the Ybus pieces the device computed from them
+struct Ybus {
+  std::vector<int> from, to;
+  std::vector<unsigned char> st, line;       // in service; counts as a line (line-loss table)
+  std::vector<double> gs, bs;                // bus shunts
+  std::vector<double> ybr, ydiag;            // [n_branch, 8] Yff Yft Ytf Ytt, [n_bus, 2]
+};
+
+// ---- 1. Ybus on the device ----
+mapdn_status ybus_on_device(mapdn_env* e, const mapdn_net_desc& net, Ybus& y) {
+  const int n = net.n_bus, nbr = net.n_branch;
+  std::vector<double> br_r(net.br_r, net.br_r + nbr), br_x(net.br_x, net.br_x + nbr);
+  std::vector<double> br_b = vec_or(net.br_b, nbr, 0.0), br_g = vec_or(net.br_g, nbr, 0.0);
+  std::vector<double> br_tap = vec_or(net.br_tap, nbr, 1.0), br_sh = vec_or(net.br_shift_deg, nbr, 0.0);
+  y.st = vec_or<unsigned char>(net.br_status, nbr, 1);
+  y.line = vec_or<unsigned char>(net.br_is_line, nbr, 1);
+  y.gs = vec_or(net.bus_gs_mw, n, 0.0); y.bs = vec_or(net.bus_bs_mvar, n, 0.0);
+  y.from.assign(net.br_from, net.br_from + nbr);
+  y.to.assign(net.br_to, net.br_to + nbr);
   for (int k = 0; k < nbr; ++k)
-    if (br_st[k] && br_r[k] == 0.0 && br_x[k] == 0.0) return bail(fail(MAPDN_ERR_INVALID, "zero-impedance branch"));
-  {
-    const double *d_r, *d_x, *d_b, *d_g, *d_tap, *d_sh, *d_gs, *d_bs;
-    const unsigned char* d_st;
-    const int *d_f, *d_t;
-    double *d_ybr, *d_ydiag;
-    TRY(dev_upload(e, br_r, &d_r)); TRY(dev_upload(e, br_x, &d_x)); TRY(dev_upload(e, br_b, &d_b));
-    TRY(dev_upload(e, br_g, &d_g)); TRY(dev_upload(e, br_tap, &d_tap)); TRY(dev_upload(e, br_sh, &d_sh));
-    TRY(dev_upload(e, br_st, &d_st)); TRY(dev_upload(e, e->br_from, &d_f)); TRY(dev_upload(e, e->br_to, &d_t));
-    TRY(dev_upload(e, gs, &d_gs)); TRY(dev_upload(e, bs, &d_bs));
-    TRY(dev_alloc(e, static_cast<size_t>(8) * nbr, &d_ybr)); TRY(dev_alloc(e, static_cast<size_t>(2) * n, &d_ydiag));
-    MAPDN_LAUNCH(ybus_branch_kernel, (nbr + 127) / 128, 128, 0, 0, nbr, d_r, d_x, d_b, d_g, d_tap, d_sh, d_st, d_ybr);
-    MAPDN_LAUNCH(ybus_diag_kernel, (n + 127) / 128, 128, 0, 0, n, nbr, d_f, d_t, d_ybr, d_gs, d_bs, 1.0 / net->base_mva, d_ydiag);
-    TRY_CUDA(cudaGetLastError());
-    e->launches += 2;
-    e->ybr.resize(static_cast<size_t>(8) * nbr);
-    e->ydiag.resize(static_cast<size_t>(2) * n);
-    TRY_CUDA(cudaMemcpy(e->ybr.data(), d_ybr, e->ybr.size() * sizeof(double), cudaMemcpyDeviceToHost));
-    TRY_CUDA(cudaMemcpy(e->ydiag.data(), d_ydiag, e->ydiag.size() * sizeof(double), cudaMemcpyDeviceToHost));
-  }
+    if (y.st[k] && br_r[k] == 0.0 && br_x[k] == 0.0) return fail(MAPDN_ERR_INVALID, "zero-impedance branch");
+  const double *d_r, *d_x, *d_b, *d_g, *d_tap, *d_sh, *d_gs, *d_bs;
+  const unsigned char* d_st;
+  const int *d_f, *d_t;
+  double *d_ybr, *d_ydiag;
+  MAPDN_TRY(dev_upload(e, br_r, &d_r)); MAPDN_TRY(dev_upload(e, br_x, &d_x)); MAPDN_TRY(dev_upload(e, br_b, &d_b));
+  MAPDN_TRY(dev_upload(e, br_g, &d_g)); MAPDN_TRY(dev_upload(e, br_tap, &d_tap)); MAPDN_TRY(dev_upload(e, br_sh, &d_sh));
+  MAPDN_TRY(dev_upload(e, y.st, &d_st)); MAPDN_TRY(dev_upload(e, y.from, &d_f)); MAPDN_TRY(dev_upload(e, y.to, &d_t));
+  MAPDN_TRY(dev_upload(e, y.gs, &d_gs)); MAPDN_TRY(dev_upload(e, y.bs, &d_bs));
+  MAPDN_TRY(dev_alloc(e, static_cast<size_t>(8) * nbr, &d_ybr)); MAPDN_TRY(dev_alloc(e, static_cast<size_t>(2) * n, &d_ydiag));
+  MAPDN_LAUNCH(ybus_branch_kernel, (nbr + 127) / 128, 128, 0, 0, nbr, d_r, d_x, d_b, d_g, d_tap, d_sh, d_st, d_ybr);
+  MAPDN_LAUNCH(ybus_diag_kernel, (n + 127) / 128, 128, 0, 0, n, nbr, d_f, d_t, d_ybr, d_gs, d_bs, 1.0 / net.base_mva, d_ydiag);
+  MAPDN_CUDA(cudaGetLastError());
+  e->launches += 2;
+  y.ybr.resize(static_cast<size_t>(8) * nbr);
+  y.ydiag.resize(static_cast<size_t>(2) * n);
+  MAPDN_CUDA(cudaMemcpy(y.ybr.data(), d_ybr, y.ybr.size() * sizeof(double), cudaMemcpyDeviceToHost));
+  MAPDN_CUDA(cudaMemcpy(y.ydiag.data(), d_ydiag, y.ydiag.size() * sizeof(double), cudaMemcpyDeviceToHost));
+  e->br_from = y.from; e->br_to = y.to; e->ybr = y.ybr; e->ydiag = y.ydiag;      // kept for the test hook
+  return MAPDN_OK;
+}
 
-  // ---- 2. symbolic analysis: merge parallel branches, check the net is radial, build the forest
-  //         of PQ buses (slack removed) and re-root every tree at its centre ----
-  struct Pair { double gab = 0, bab = 0, gba = 0, bba = 0; };   // Y[a,b], Y[b,a] with a < b
-  std::map<std::pair<int, int>, Pair> pairs;
-  for (int k = 0; k < nbr; ++k) {
-    if (!br_st[k]) continue;
-    const int f = e->br_from[k], t = e->br_to[k];
-    const double* y = &e->ybr[8 * static_cast<size_t>(k)];
-    Pair& pr = pairs[{std::min(f, t), std::max(f, t)}];
-    if (f < t) { pr.gab += y[2]; pr.bab += y[3]; pr.gba += y[4]; pr.bba += y[5]; }   // Ybus[f,t]+=Yft, [t,f]+=Ytf
-    else       { pr.gba += y[2]; pr.bba += y[3]; pr.gab += y[4]; pr.bab += y[5]; }
+struct Pair { double gab = 0, bab = 0, gba = 0, bba = 0; };   // Y[a,b], Y[b,a] with a < b
+using Pairs = std::map<std::pair<int, int>, Pair>;            // the in-service branches, parallel ones merged
+
+// Ybus[a,b] of two different buses; zero when no branch joins them
+void yoff(const Pairs& pairs, int a, int b, double& g, double& bb) {
+  const auto it = pairs.find({std::min(a, b), std::max(a, b)});
+  if (it == pairs.end()) { g = bb = 0.0; return; }
+  const Pair& pr = it->second;
+  if (a < b) { g = pr.gab; bb = pr.bab; } else { g = pr.gba; bb = pr.bba; }
+}
+
+// The forest of PQ buses. Nodes are numbered breadth first (roots, then level by level) until relabel_nodes permutes them:
+// it rewrites order, node_of_bus, parent, nchild, kid0 and kid1; cfirst, height, eorder, elev and dlev describe the
+// breadth-first numbering, which the sweep schedules are planned on.
+struct Forest {
+  int n = 0, npq = 0, slack = 0;
+  Pairs pairs;
+  std::vector<std::vector<int>> adj;         // by bus, sorted
+  bool meshed = false;
+  std::vector<int> order, node_of_bus, parent_bus;    // node -> bus; bus -> node (slack -> npq); bus -> parent bus (-1: root)
+  std::vector<int> parent, nchild, cfirst, height;    // by node; the children of i are cfirst[i] .. cfirst[i] + nchild[i] - 1
+  std::vector<int> kid0, kid1;               // first and second child (npq = none); further children follow kid1 contiguously
+  std::vector<int> eorder;                   // nodes by height
+  std::vector<uint16_t> elev, dlev;          // [n_lev + 1] level starts: in eorder by height, in node ids by depth
+  int n_lev = 0, max_children = 0;
+};
+
+// ---- 2. symbolic analysis: merge parallel branches, check the net is radial, build the forest
+//         of PQ buses (slack removed) and re-root every tree at its centre ----
+mapdn_status build_forest(const Ybus& y, int n, int slack, Forest& f) {
+  const int npq = n - 1;
+  f.n = n; f.npq = npq; f.slack = slack;
+  Pairs& pairs = f.pairs;
+  for (size_t k = 0; k < y.from.size(); ++k) {
+    if (!y.st[k]) continue;
+    const int fr = y.from[k], t = y.to[k];
+    const double* yk = &y.ybr[8 * k];
+    Pair& pr = pairs[{std::min(fr, t), std::max(fr, t)}];
+    if (fr < t) { pr.gab += yk[2]; pr.bab += yk[3]; pr.gba += yk[4]; pr.bba += yk[5]; }   // Ybus[f,t]+=Yft, [t,f]+=Ytf
+    else        { pr.gba += yk[2]; pr.bba += yk[3]; pr.gab += yk[4]; pr.bab += yk[5]; }
   }
-  auto yoff = [&](int a, int b, double& g, double& bb) {          // Ybus[a,b]
-    const Pair& pr = pairs[{std::min(a, b), std::max(a, b)}];
-    if (a < b) { g = pr.gab; bb = pr.bab; } else { g = pr.gba; bb = pr.bba; }
-  };
-  const int slack = net->slack_bus;
-  std::vector<std::vector<int>> adj(n);
+  std::vector<std::vector<int>>& adj = f.adj;
+  adj.resize(n);
   for (auto& kv : pairs) { adj[kv.first.first].push_back(kv.first.second); adj[kv.first.second].push_back(kv.first.first); }
   for (auto& a : adj) std::sort(a.begin(), a.end());
   {   // connectivity + radiality on the full graph
@@ -538,16 +556,15 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
     for (size_t qh = 0; qh < q.size(); ++qh)
       for (int v : adj[q[qh]]) if (!seen[v]) { seen[v] = 1; q.push_back(v); }
     if (static_cast<int>(q.size()) != n)
-      return bail(fail(MAPDN_ERR_TOPOLOGY, "network is not connected to the slack bus (" +
-                                               std::to_string(n - q.size()) + " unreachable buses)"));
+      return fail(MAPDN_ERR_TOPOLOGY, "network is not connected to the slack bus (" +
+                                          std::to_string(n - q.size()) + " unreachable buses)");
   }
   // A radial net (|edges| = n - 1) takes the zero-fill tree solver; a meshed one the dense-LU fallback.
-  const bool meshed = static_cast<int>(pairs.size()) != n - 1;
+  const bool meshed = f.meshed = static_cast<int>(pairs.size()) != n - 1;
   if (meshed && n - 1 > 256)
-    return bail(fail(MAPDN_ERR_TOPOLOGY, "network is meshed (" + std::to_string(pairs.size() - (n - 1)) +
-                                             " loop-closing branches) and has more than 256 PQ buses: the dense "
-                                             "fallback solver only covers small meshed feeders"));
-  const int npq = n - 1;
+    return fail(MAPDN_ERR_TOPOLOGY, "network is meshed (" + std::to_string(pairs.size() - (n - 1)) +
+                                        " loop-closing branches) and has more than 256 PQ buses: the dense "
+                                        "fallback solver only covers small meshed feeders");
   // BFS inside the PQ forest (never crossing the slack bus)
   auto bfs = [&](int src, std::vector<int>& dist, std::vector<int>& from) {
     std::vector<int> q{src};
@@ -571,7 +588,9 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
       roots.push_back(c);
     }
   }
-  std::vector<int> order, node_of_bus(n, -1), parent_bus(n, -1), depth(n, 0);
+  std::vector<int>&order = f.order, &node_of_bus = f.node_of_bus, &parent_bus = f.parent_bus;
+  std::vector<int> depth(n, 0);
+  node_of_bus.assign(n, -1); parent_bus.assign(n, -1);
   order.reserve(npq);
   for (int r : roots) { node_of_bus[r] = static_cast<int>(order.size()); order.push_back(r); }
   for (size_t qh = 0; qh < order.size(); ++qh) {
@@ -585,7 +604,8 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
     }
   }
   node_of_bus[slack] = npq;
-  std::vector<int> parent(npq, -1), nchild(npq, 0), height(npq, 0);
+  std::vector<int>&parent = f.parent, &nchild = f.nchild, &height = f.height, &cfirst = f.cfirst;
+  parent.assign(npq, -1); nchild.assign(npq, 0); height.assign(npq, 0);
   for (int i = 0; i < npq; ++i)
     if (parent_bus[order[i]] >= 0) { parent[i] = node_of_bus[parent_bus[order[i]]]; nchild[parent[i]]++; }
   if (meshed) {   // no elimination forest: every bus is its own root, the sweeps are not used
@@ -595,309 +615,350 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
   }
   for (int i = npq - 1; i >= 0; --i)
     if (parent[i] >= 0) height[parent[i]] = std::max(height[parent[i]], height[i] + 1);
-  std::vector<int> cfirst(npq + 1);
+  cfirst.resize(npq + 1);
   cfirst[0] = static_cast<int>(roots.size());
   for (int i = 0; i < npq; ++i) cfirst[i + 1] = cfirst[i] + nchild[i];
   int max_h = 0;
   for (int i = 0; i < npq; ++i) max_h = std::max(max_h, height[i]);
-  const int n_lev = max_h + 1;                          // = max depth + 1
-  std::vector<uint16_t> elev(n_lev + 1), dlev(n_lev + 1);
-  std::vector<int> eorder;
+  const int n_lev = f.n_lev = max_h + 1;                // = max depth + 1
+  f.elev.resize(n_lev + 1); f.dlev.resize(n_lev + 1);
   for (int hgt = 0; hgt <= max_h; ++hgt) {
-    elev[hgt] = static_cast<uint16_t>(eorder.size());
-    for (int i = 0; i < npq; ++i) if (height[i] == hgt) eorder.push_back(i);
+    f.elev[hgt] = static_cast<uint16_t>(f.eorder.size());
+    for (int i = 0; i < npq; ++i) if (height[i] == hgt) f.eorder.push_back(i);
   }
-  elev[n_lev] = static_cast<uint16_t>(eorder.size());
+  f.elev[n_lev] = static_cast<uint16_t>(f.eorder.size());
   {
     int d = 0;
-    dlev[0] = 0;
-    for (int i = 0; i < npq; ++i) while (depth[order[i]] > d) dlev[++d] = static_cast<uint16_t>(i);
-    while (d < n_lev) dlev[++d] = static_cast<uint16_t>(npq);
+    f.dlev[0] = 0;
+    for (int i = 0; i < npq; ++i) while (depth[order[i]] > d) f.dlev[++d] = static_cast<uint16_t>(i);
+    while (d < n_lev) f.dlev[++d] = static_cast<uint16_t>(npq);
   }
-  int max_children = 0;
-  for (int i = 0; i < npq; ++i) max_children = std::max(max_children, nchild[i]);
-  int G = cfg->lanes_per_env;
+  f.kid0.assign(npq, npq); f.kid1.assign(npq, npq);
+  for (int i = 0; i < npq; ++i) {
+    f.max_children = std::max(f.max_children, nchild[i]);
+    if (nchild[i] > 0) f.kid0[i] = cfirst[i];
+    if (nchild[i] > 1) f.kid1[i] = cfirst[i] + 1;
+  }
+  return MAPDN_OK;
+}
+
+// Idle lanes of a sweep step work on the trash record npq + 1 and reach for the zero slot npq
+uint64_t esched_idle(int npq) {
+  return static_cast<uint64_t>(npq + 1) | (static_cast<uint64_t>(npq) << 16) | (static_cast<uint64_t>(npq) << 32) |
+         (static_cast<uint64_t>(kEschedReg0 | kEschedIdle) << 48);
+}
+uint64_t bsched_idle(int npq) {
+  return static_cast<uint64_t>(npq + 1) | (static_cast<uint64_t>(npq) << 16) |
+         (static_cast<uint64_t>(kBschedRegParent | kBschedIdle) << 32);
+}
+
+struct Sweeps {
+  int G = 0;                                 // lanes per env
+  std::vector<uint64_t> esched, bsched;      // [steps * G] forward elimination / back substitution, see kernel_params.h
+  int n_wide_e = 0, n_narrow_b = 0;          // G > 32: forward steps [n_wide_e, end) and back steps [0, n_narrow_b) use warp 0 only
+  int n_esteps() const { return static_cast<int>(esched.size()) / G; }
+  int n_bsteps() const { return static_cast<int>(bsched.size()) / G; }
+};
+
+// ---- 2a. lanes per env and the two sweep schedules ----
+mapdn_status plan_sweeps(const Forest& f, int lanes_per_env, Sweeps& s) {
+  const int npq = f.npq, n_lev = f.n_lev;
+  const std::vector<int>&nchild = f.nchild, &cfirst = f.cfirst, &height = f.height, &parent = f.parent;
+  int G = lanes_per_env;
   if (G == 0) G = (npq <= 64) ? 8 : (npq <= 256 ? 32 : 64);      // fastest on H100 at every BASELINE size (DESIGN.md §4)
-  if (meshed) G = 32;                    // the dense fallback works one warp per env
+  if (f.meshed) G = 32;                  // the dense fallback works one warp per env
+  s.G = G;
   // Flat schedules for this G: a level wider than G takes several steps; idle lanes get the trash record.
   // Lanes follow chains: a bus is placed on the lane that handled its child (forward sweep) / its parent
   // (back sweep) in the immediately preceding step whenever that lane is free, so the dependent value can
   // stay in registers.
-  const int trash = npq + 1;
-  std::vector<uint64_t> esched, bsched;
-  int n_wide_e = 0, n_narrow_b = 0;      // G > 32: forward steps [n_wide_e, end) and back steps [0, n_narrow_b) use warp 0 only
-  {
-    std::vector<int> lane_of(npq, -1), step_of(npq, -1), reg_child(npq, -1), epos(npq, -1);
-    int cur = 0;
-    // Multi-warp groups (G > 32): the levels near the roots hold a handful of buses. From the first level on after which no
-    // level is wider than a warp ("narrow suffix" of the forward sweep / "narrow prefix" of the back sweep) only warp 0 of
-    // the group works: those steps are packed into lanes 0..31 and synchronise with __syncwarp instead of a named barrier.
-    int first_narrow_lev = n_lev;
-    if (G > 32) { while (first_narrow_lev > 0 && elev[first_narrow_lev] - elev[first_narrow_lev - 1] <= 32) --first_narrow_lev; }
-    n_wide_e = -1;
-    for (int l = 0; l < n_lev; ++l) {
-      const int w = elev[l + 1] - elev[l], nst = (w + G - 1) / G;
-      const bool narrow = G > 32 && l >= first_narrow_lev;
-      if (narrow && n_wide_e < 0) n_wide_e = cur;
-      std::vector<int> slot(static_cast<size_t>(nst) * G, -1), inh(npq, -1);
-      std::vector<int> rest;
-      for (int k = elev[l]; k < elev[l + 1]; ++k) {
-        const int i = eorder[k];
-        int pick = -1;
-        if (nchild[i] >= 1 && nchild[i] <= 2)
-          for (int c = cfirst[i]; c < cfirst[i] + nchild[i]; ++c)
-            if (step_of[c] == cur - 1 && slot[lane_of[c]] < 0 && (!narrow || lane_of[c] < 32) &&
-                (pick < 0 || height[c] > height[pick])) pick = c;
-        if (pick >= 0) { slot[lane_of[pick]] = i; inh[i] = pick; }
-        else rest.push_back(i);
-      }
-      size_t pos = 0;
-      for (int i : rest) { while (slot[pos] >= 0) ++pos; slot[pos] = i; }
-      for (int sidx = 0; sidx < nst * G; ++sidx) {
-        const int i = slot[sidx];
-        if (i < 0) { esched.push_back(static_cast<uint64_t>(trash) | (static_cast<uint64_t>(npq) << 16) |
-                                      (static_cast<uint64_t>(npq) << 32) | (static_cast<uint64_t>(kEschedReg0 | kEschedIdle) << 48)); continue; }
-        lane_of[i] = sidx % G; step_of[i] = cur + sidx / G;
-        uint64_t c0 = npq, c1 = npq, fl = kEschedLeaf;       // no child: zero update, nothing to fetch
-        if (nchild[i] > 2) {
-          c0 = cfirst[i]; c1 = cfirst[i] + 1; fl = static_cast<uint64_t>(std::min(nchild[i] - 2, 255)) | kEschedLoad0 | kEschedLoad1;
-          if (nchild[i] - 2 > 255) return bail(fail(MAPDN_ERR_UNSUPPORTED, "a bus with more than 257 children"));
-        } else if (nchild[i] >= 1) {
-          const int a0 = inh[i] >= 0 ? inh[i] : cfirst[i];
-          c0 = a0; fl = (inh[i] >= 0 && sidx / G == 0) ? kEschedReg0 : kEschedLoad0;
-          if (fl & kEschedReg0) reg_child[i] = a0;
-          if (nchild[i] == 2) { c1 = (a0 == cfirst[i]) ? cfirst[i] + 1 : cfirst[i]; fl |= kEschedLoad1; }
-        }
-        epos[i] = static_cast<int>(esched.size());
-        esched.push_back(static_cast<uint64_t>(i) | (c0 << 16) | (c1 << 32) | (fl << 48));
-      }
-      cur += nst;
+  const uint64_t trash = npq + 1;
+  std::vector<uint64_t>&esched = s.esched, &bsched = s.bsched;
+  std::vector<int> lane_of(npq, -1), step_of(npq, -1), reg_child(npq, -1), epos(npq, -1);
+  int cur = 0;
+  // Multi-warp groups (G > 32): the levels near the roots hold a handful of buses. From the first level on after which no
+  // level is wider than a warp ("narrow suffix" of the forward sweep / "narrow prefix" of the back sweep) only warp 0 of
+  // the group works: those steps are packed into lanes 0..31 and synchronise with __syncwarp instead of a named barrier.
+  int first_narrow_lev = n_lev;
+  if (G > 32) { while (first_narrow_lev > 0 && f.elev[first_narrow_lev] - f.elev[first_narrow_lev - 1] <= 32) --first_narrow_lev; }
+  s.n_wide_e = -1;
+  for (int l = 0; l < n_lev; ++l) {
+    const int w = f.elev[l + 1] - f.elev[l], nst = (w + G - 1) / G;
+    const bool narrow = G > 32 && l >= first_narrow_lev;
+    if (narrow && s.n_wide_e < 0) s.n_wide_e = cur;
+    std::vector<int> slot(static_cast<size_t>(nst) * G, -1), inh(npq, -1);
+    std::vector<int> rest;
+    for (int k = f.elev[l]; k < f.elev[l + 1]; ++k) {
+      const int i = f.eorder[k];
+      int pick = -1;
+      if (nchild[i] >= 1 && nchild[i] <= 2)
+        for (int c = cfirst[i]; c < cfirst[i] + nchild[i]; ++c)
+          if (step_of[c] == cur - 1 && slot[lane_of[c]] < 0 && (!narrow || lane_of[c] < 32) &&
+              (pick < 0 || height[c] > height[pick])) pick = c;
+      if (pick >= 0) { slot[lane_of[pick]] = i; inh[i] = pick; }
+      else rest.push_back(i);
     }
-    // a bus stores its Schur update only if its parent will fetch it from shared memory
-    for (int i = 0; i < npq; ++i)
-      if (parent[i] >= 0 && reg_child[parent[i]] != i) esched[epos[i]] |= static_cast<uint64_t>(kEschedStore) << 48;
-    if (n_wide_e < 0) n_wide_e = cur;             // no narrow suffix
-    // back sweep by depth: children inherit the lane of their parent (the child with the tallest subtree first)
-    std::fill(lane_of.begin(), lane_of.end(), -1); std::fill(step_of.begin(), step_of.end(), -1);
-    cur = 0;
-    const int first_back_level = 1;      // the roots' dx = D^-1 r is already in place
-    int last_narrow_dlev = first_back_level - 1;  // depth levels first_back_level .. last_narrow_dlev are narrow (prefix)
-    if (G > 32) { while (last_narrow_dlev + 1 < n_lev && dlev[last_narrow_dlev + 2] - dlev[last_narrow_dlev + 1] <= 32) ++last_narrow_dlev; }
-    n_narrow_b = 0;
-    for (int l = first_back_level; l < n_lev; ++l) {
-      const int w = dlev[l + 1] - dlev[l], nst = (w + G - 1) / G;
-      if (G > 32 && l <= last_narrow_dlev) n_narrow_b = cur + nst;
-      std::vector<int> slot(static_cast<size_t>(nst) * G, -1);
-      std::vector<char> reg(npq, 0);
-      std::vector<int> nodes;
-      for (int i = dlev[l]; i < dlev[l + 1]; ++i) nodes.push_back(i);
-      std::stable_sort(nodes.begin(), nodes.end(), [&](int a, int b) { return height[a] > height[b]; });
-      std::vector<int> rest;
-      for (int i : nodes) {
-        const int pa = parent[i];
-        if (pa >= 0 && step_of[pa] == cur - 1 && lane_of[pa] >= 0 && slot[lane_of[pa]] < 0) { slot[lane_of[pa]] = i; reg[i] = 1; }
-        else rest.push_back(i);
+    size_t pos = 0;
+    for (int i : rest) { while (slot[pos] >= 0) ++pos; slot[pos] = i; }
+    for (int sidx = 0; sidx < nst * G; ++sidx) {
+      const int i = slot[sidx];
+      if (i < 0) { esched.push_back(esched_idle(npq)); continue; }
+      lane_of[i] = sidx % G; step_of[i] = cur + sidx / G;
+      uint64_t c0 = npq, c1 = npq, fl = kEschedLeaf;       // no child: zero update, nothing to fetch
+      if (nchild[i] > 2) {
+        c0 = cfirst[i]; c1 = cfirst[i] + 1; fl = static_cast<uint64_t>(std::min(nchild[i] - 2, 255)) | kEschedLoad0 | kEschedLoad1;
+        if (nchild[i] - 2 > 255) return fail(MAPDN_ERR_UNSUPPORTED, "a bus with more than 257 children");
+      } else if (nchild[i] >= 1) {
+        const int a0 = inh[i] >= 0 ? inh[i] : cfirst[i];
+        c0 = a0; fl = (inh[i] >= 0 && sidx / G == 0) ? kEschedReg0 : kEschedLoad0;
+        if (fl & kEschedReg0) reg_child[i] = a0;
+        if (nchild[i] == 2) { c1 = (a0 == cfirst[i]) ? cfirst[i] + 1 : cfirst[i]; fl |= kEschedLoad1; }
       }
-      size_t pos = 0;
-      for (int i : rest) { while (slot[pos] >= 0) ++pos; slot[pos] = i; }
-      for (int sidx = 0; sidx < nst * G; ++sidx) {
-        const int i = slot[sidx];
-        if (i < 0) {
-          bsched.push_back(static_cast<uint64_t>(trash) | (static_cast<uint64_t>(npq) << 16) |
-                           (static_cast<uint64_t>(kBschedRegParent | kBschedIdle) << 32));
-          continue;
-        }
-        lane_of[i] = sidx % G; step_of[i] = cur + sidx / G;
-        bsched.push_back(static_cast<uint64_t>(i) | (static_cast<uint64_t>(parent[i] >= 0 ? parent[i] : npq) << 16) |
-                         (static_cast<uint64_t>((reg[i] && sidx / G == 0) ? kBschedRegParent : 0u) << 32));
-      }
-      cur += nst;
+      epos[i] = static_cast<int>(esched.size());
+      esched.push_back(static_cast<uint64_t>(i) | (c0 << 16) | (c1 << 32) | (fl << 48));
     }
+    cur += nst;
+  }
+  // a bus stores its Schur update only if its parent will fetch it from shared memory
+  for (int i = 0; i < npq; ++i)
+    if (parent[i] >= 0 && reg_child[parent[i]] != i) esched[epos[i]] |= static_cast<uint64_t>(kEschedStore) << 48;
+  if (s.n_wide_e < 0) s.n_wide_e = cur;           // no narrow suffix
+  // back sweep by depth: children inherit the lane of their parent (the child with the tallest subtree first)
+  std::fill(lane_of.begin(), lane_of.end(), -1); std::fill(step_of.begin(), step_of.end(), -1);
+  cur = 0;
+  const int first_back_level = 1;      // the roots' dx = D^-1 r is already in place
+  int last_narrow_dlev = first_back_level - 1;  // depth levels first_back_level .. last_narrow_dlev are narrow (prefix)
+  if (G > 32) { while (last_narrow_dlev + 1 < n_lev && f.dlev[last_narrow_dlev + 2] - f.dlev[last_narrow_dlev + 1] <= 32) ++last_narrow_dlev; }
+  s.n_narrow_b = 0;
+  for (int l = first_back_level; l < n_lev; ++l) {
+    const int w = f.dlev[l + 1] - f.dlev[l], nst = (w + G - 1) / G;
+    if (G > 32 && l <= last_narrow_dlev) s.n_narrow_b = cur + nst;
+    std::vector<int> slot(static_cast<size_t>(nst) * G, -1);
+    std::vector<char> reg(npq, 0);
+    std::vector<int> nodes;
+    for (int i = f.dlev[l]; i < f.dlev[l + 1]; ++i) nodes.push_back(i);
+    std::stable_sort(nodes.begin(), nodes.end(), [&](int a, int b) { return height[a] > height[b]; });
+    std::vector<int> rest;
+    for (int i : nodes) {
+      const int pa = parent[i];
+      if (pa >= 0 && step_of[pa] == cur - 1 && lane_of[pa] >= 0 && slot[lane_of[pa]] < 0) { slot[lane_of[pa]] = i; reg[i] = 1; }
+      else rest.push_back(i);
+    }
+    size_t pos = 0;
+    for (int i : rest) { while (slot[pos] >= 0) ++pos; slot[pos] = i; }
+    for (int sidx = 0; sidx < nst * G; ++sidx) {
+      const int i = slot[sidx];
+      if (i < 0) { bsched.push_back(bsched_idle(npq)); continue; }
+      lane_of[i] = sidx % G; step_of[i] = cur + sidx / G;
+      bsched.push_back(static_cast<uint64_t>(i) | (static_cast<uint64_t>(parent[i] >= 0 ? parent[i] : npq) << 16) |
+                       (static_cast<uint64_t>((reg[i] && sidx / G == 0) ? kBschedRegParent : 0u) << 32));
+    }
+    cur += nst;
   }
   if (getenv("MAPDN_DEBUG_SCHED")) {
     int nreg = 0, nl0 = 0, nl1 = 0, nreal = 0;
-    for (uint64_t e2 : esched) { if ((e2 & 0xFFFF) == (uint64_t)trash) continue; ++nreal; unsigned fl = e2 >> 48; nreg += !!(fl & kEschedReg0); nl0 += !!(fl & kEschedLoad0); nl1 += !!(fl & kEschedLoad1); }
+    for (uint64_t e2 : esched) { if ((e2 & 0xFFFF) == trash) continue; ++nreal; unsigned fl = e2 >> 48; nreg += !!(fl & kEschedReg0); nl0 += !!(fl & kEschedLoad0); nl1 += !!(fl & kEschedLoad1); }
     int breg = 0, breal = 0;
-    for (uint64_t b2 : bsched) { if ((b2 & 0xFFFF) == (uint64_t)trash) continue; ++breal; breg += (b2 >> 32) & 1; }
+    for (uint64_t b2 : bsched) { if ((b2 & 0xFFFF) == trash) continue; ++breal; breg += (b2 >> 32) & 1; }
     fprintf(stderr, "[sched] G=%d levels=%d esteps=%zu real=%d reg0=%d load0=%d load1=%d | bsteps=%zu real=%d regp=%d\n", G, n_lev,
             esched.size() / G, nreal, nreg, nl0, nl1, bsched.size() / G, breal, breg);
   }
-  if (bsched.empty())      // a forest of single buses: one all-idle step
-    bsched.assign(G, static_cast<uint64_t>(trash) | (static_cast<uint64_t>(npq) << 16) |
-                         (static_cast<uint64_t>(kBschedRegParent | kBschedIdle) << 32));
-  const int n_esteps = static_cast<int>(esched.size()) / G, n_bsteps = static_cast<int>(bsched.size()) / G;
+  if (bsched.empty()) bsched.assign(G, bsched_idle(npq));      // a forest of single buses: one all-idle step
+  return MAPDN_OK;
+}
 
-  // ---- 2b. bank-conflict-aware relabelling of the node records ----
-  // A node record is 144 B = 9 x 16 B, so the 16-byte bank group of field f of node i is (i + f) mod 8: the eight lanes of a
-  // quarter-warp (one 128-bit access wavefront) are conflict free iff their node ids differ mod 8. The passes own nodes
-  // by id (conflict free by construction) but reach parents / children by pointer, and the sweeps touch whatever the
-  // schedules say; ncu counted 25 % of the shared-load wavefronts as conflicts with the breadth-first ids. The ids are
-  // free to choose, so pick a permutation that minimises the weighted number of extra wavefronts over every access group
-  // of the kernel (simulated annealing on pairwise swaps, deterministic; identity when it does not apply).
-  std::vector<int> kid0(npq, npq), kid1(npq, npq);
-  for (int i = 0; i < npq; ++i) { if (nchild[i] > 0) kid0[i] = cfirst[i]; if (nchild[i] > 1) kid1[i] = cfirst[i] + 1; }
-  double relabel_cost0 = 0.0, relabel_cost1 = 0.0;
-  if (!meshed && max_children <= 2 && G >= 8 && npq >= 8 && !getenv("MAPDN_NO_RELABEL")) {
-    struct Grp { std::vector<int> nodes; double w; };
-    std::vector<Grp> groups;                                  // groups whose members do not depend on the labelling
-    const double w_iter = 4.5;                                // Newton iterations per step (sweeps and passes run that often)
-    auto add_quarters = [&](const std::vector<int>& per_lane, double w) {      // per_lane: node per lane of the group (-1: no access)
-      for (int q = 0; q < G / 8; ++q) {
-        Grp g; g.w = w;
-        for (int l = 8 * q; l < 8 * q + 8; ++l) if (per_lane[l] >= 0) g.nodes.push_back(per_lane[l]);
-        std::sort(g.nodes.begin(), g.nodes.end());
-        g.nodes.erase(std::unique(g.nodes.begin(), g.nodes.end()), g.nodes.end());      // same address = broadcast
-        if (g.nodes.size() > 1) groups.push_back(std::move(g));
-      }
-    };
-    std::vector<int> own(G), c0v(G), c1v(G);
-    for (size_t st = 0; st < esched.size() / G; ++st) {
-      for (int l = 0; l < G; ++l) {
-        const uint64_t ed = esched[st * G + l];
-        const unsigned fl = static_cast<unsigned>(ed >> 48);
-        own[l] = static_cast<int>(ed & 0xFFFFu);
-        c0v[l] = (fl & kEschedLoad0) ? static_cast<int>((ed >> 16) & 0xFFFFu) : -1;
-        c1v[l] = (fl & kEschedLoad1) ? static_cast<int>((ed >> 32) & 0xFFFFu) : -1;
-      }
-      add_quarters(own, 2.0 * w_iter);                        // own blocks: loaded (prefetch) and stored
-      add_quarters(c0v, w_iter); add_quarters(c1v, w_iter);
+// ---- 2b. bank-conflict-aware relabelling of the node records ----
+// A node record is 144 B = 9 x 16 B, so the 16-byte bank group of field f of node i is (i + f) mod 8: the eight lanes of a
+// quarter-warp (one 128-bit access wavefront) are conflict free iff their node ids differ mod 8. The passes own nodes
+// by id (conflict free by construction) but reach parents / children by pointer, and the sweeps touch whatever the
+// schedules say; ncu counted 25 % of the shared-load wavefronts as conflicts with the breadth-first ids. The ids are
+// free to choose, so pick a permutation that minimises the weighted number of extra wavefronts over every access group
+// of the kernel (simulated annealing on pairwise swaps, deterministic; identity when it does not apply).
+// Permutes the forest and both schedules together, or leaves them as they are.
+void relabel_nodes(const Ybus& y, Forest& f, Sweeps& s) {
+  const int n = f.n, npq = f.npq, G = s.G;
+  std::vector<int>&order = f.order, &node_of_bus = f.node_of_bus, &parent = f.parent, &nchild = f.nchild, &kid0 = f.kid0, &kid1 = f.kid1;
+  std::vector<uint64_t>&esched = s.esched, &bsched = s.bsched;
+  if (f.meshed || f.max_children > 2 || G < 8 || npq < 8 || getenv("MAPDN_NO_RELABEL")) return;
+  struct Grp { std::vector<int> nodes; double w; };
+  std::vector<Grp> groups;                                  // groups whose members do not depend on the labelling
+  const double w_iter = 4.5;                                // Newton iterations per step (sweeps and passes run that often)
+  auto add_quarters = [&](const std::vector<int>& per_lane, double w) {      // per_lane: node per lane of the group (-1: no access)
+    for (int q = 0; q < G / 8; ++q) {
+      Grp g; g.w = w;
+      for (int l = 8 * q; l < 8 * q + 8; ++l) if (per_lane[l] >= 0) g.nodes.push_back(per_lane[l]);
+      std::sort(g.nodes.begin(), g.nodes.end());
+      g.nodes.erase(std::unique(g.nodes.begin(), g.nodes.end()), g.nodes.end());      // same address = broadcast
+      if (g.nodes.size() > 1) groups.push_back(std::move(g));
     }
-    for (size_t st = 0; st < bsched.size() / G; ++st) {
-      for (int l = 0; l < G; ++l) {
-        const uint64_t bd = bsched[st * G + l];
-        const unsigned bfl = static_cast<unsigned>(bd >> 32);
-        own[l] = static_cast<int>(bd & 0xFFFFu);
-        c0v[l] = (bfl & (kBschedRegParent | kBschedIdle)) ? -1 : static_cast<int>((bd >> 16) & 0xFFFFu);
-      }
-      add_quarters(own, 2.0 * w_iter); add_quarters(c0v, w_iter);
+  };
+  std::vector<int> own(G), c0v(G), c1v(G);
+  for (size_t st = 0; st < esched.size() / G; ++st) {
+    for (int l = 0; l < G; ++l) {
+      const uint64_t ed = esched[st * G + l];
+      const unsigned fl = static_cast<unsigned>(ed >> 48);
+      own[l] = static_cast<int>(ed & 0xFFFFu);
+      c0v[l] = (fl & kEschedLoad0) ? static_cast<int>((ed >> 16) & 0xFFFFu) : -1;
+      c1v[l] = (fl & kEschedLoad1) ? static_cast<int>((ed >> 32) & 0xFFFFu) : -1;
     }
-    for (int b0 = 0; b0 < n; b0 += G) {                       // epilogue: per-bus loop, buses b0 + lane
-      for (int l = 0; l < G; ++l) own[l] = (b0 + l < n) ? node_of_bus[b0 + l] : -1;
-      add_quarters(own, 1.0);
-    }
-    {
-      std::vector<int> lf, lt;
-      for (int k = 0; k < nbr; ++k) if (br_line[k]) { lf.push_back(node_of_bus[e->br_from[k]]); lt.push_back(node_of_bus[e->br_to[k]]); }
-      for (size_t k0 = 0; k0 < lf.size(); k0 += G) {
-        for (int l = 0; l < G; ++l) { own[l] = (k0 + l < lf.size()) ? lf[k0 + l] : -1; c0v[l] = (k0 + l < lt.size()) ? lt[k0 + l] : -1; }
-        add_quarters(own, 1.0); add_quarters(c0v, 1.0);
-      }
-    }
-    // lab[base id] = label; sentinel / trash keep their ids
-    std::vector<int> lab(npq + 2), inv(npq + 2);
-    for (int i = 0; i < npq + 2; ++i) lab[i] = inv[i] = i;
-    auto extra = [&](const int* ids, int cnt) {               // extra wavefronts of one access: max multiplicity - 1
-      int c[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-      int mx = 0;
-      for (int k = 0; k < cnt; ++k) mx = std::max(mx, ++c[ids[k] & 7]);
-      return std::max(0, mx - 1);
-    };
-    auto cost = [&]() {
-      double tot = 0.0;
-      int ids[8];
-      for (const Grp& g : groups) {
-        int cnt = 0;
-        for (int v : g.nodes) ids[cnt++] = lab[v];
-        tot += g.w * extra(ids, cnt);
-      }
-      // passes: label L is handled by lane L % G in round L / G; neighbours reached by pointer
-      for (int L0 = 0; L0 < npq; L0 += 8) {
-        int pa[8], k0[8], k1[8], np = 0, n0 = 0, n1 = 0;
-        auto push_unique = [](int* a, int& cnt, int v) { for (int k = 0; k < cnt; ++k) if (a[k] == v) return; a[cnt++] = v; };
-        for (int L = L0; L < std::min(npq, L0 + 8); ++L) {
-          const int i = inv[L];
-          push_unique(pa, np, parent[i] >= 0 ? lab[parent[i]] : npq);
-          push_unique(k0, n0, lab[kid0[i]]); push_unique(k1, n1, lab[kid1[i]]);
-        }
-        tot += w_iter * (extra(pa, np) + extra(k0, n0) + extra(k1, n1));
-      }
-      return tot;
-    };
-    relabel_cost0 = cost();
-    double cur = relabel_cost0, best = cur;
-    std::vector<int> best_lab = lab;
-    uint64_t rng = 0x9E3779B97F4A7C15ull;
-    auto rnd = [&]() { rng ^= rng << 13; rng ^= rng >> 7; rng ^= rng << 17; return rng; };
-    const int iters = std::min(400 * npq, 30000);
-    double T = std::max(1.0, 0.02 * cur);
-    const double cool = std::pow(1e-3, 1.0 / std::max(1, iters));
-    for (int it = 0; it < iters && best > 0.0; ++it, T *= cool) {
-      const int a = static_cast<int>(rnd() % npq), b = static_cast<int>(rnd() % npq);
-      if (a == b || ((lab[a] ^ lab[b]) & 7) == 0) continue;  // same residue: no effect on any group
-      std::swap(lab[a], lab[b]); inv[lab[a]] = a; inv[lab[b]] = b;
-      const double c2 = cost();
-      const double u = static_cast<double>(rnd() >> 11) * (1.0 / 9007199254740992.0);
-      if (c2 <= cur || u < std::exp((cur - c2) / T)) {
-        cur = c2;
-        if (cur < best) { best = cur; best_lab = lab; }
-      } else {
-        std::swap(lab[a], lab[b]); inv[lab[a]] = a; inv[lab[b]] = b;
-      }
-    }
-    lab = best_lab;
-    relabel_cost1 = best;
-    if (best < relabel_cost0) {
-      // apply: new id of base node i is lab[i]
-      std::vector<int> order2(npq), parent2(npq), nchild2(npq), k0b(npq), k1b(npq);
-      for (int i = 0; i < npq; ++i) {
-        const int L = lab[i];
-        order2[L] = order[i];
-        parent2[L] = parent[i] >= 0 ? lab[parent[i]] : -1;
-        nchild2[L] = nchild[i];
-        k0b[L] = lab[kid0[i]]; k1b[L] = lab[kid1[i]];
-      }
-      order = order2; parent = parent2; nchild = nchild2; kid0 = k0b; kid1 = k1b;
-      for (int i = 0; i < npq; ++i) node_of_bus[order[i]] = i;
-      auto map16 = [&](uint64_t v) { return static_cast<uint64_t>(lab[static_cast<int>(v & 0xFFFFu)]); };
-      for (uint64_t& ed : esched)
-        ed = (ed & 0xFFFF000000000000ull) | map16(ed) | (map16(ed >> 16) << 16) | (map16(ed >> 32) << 32);
-      for (uint64_t& bd : bsched)
-        bd = (bd & 0xFFFFFFFF00000000ull) | map16(bd) | (map16(bd >> 16) << 16);
-    }
-    if (getenv("MAPDN_DEBUG_SCHED"))
-      fprintf(stderr, "[relabel] weighted extra shared-memory wavefronts per env-step: %.1f -> %.1f (%d swaps tried)\n",
-              relabel_cost0, relabel_cost1, iters);
+    add_quarters(own, 2.0 * w_iter);                        // own blocks: loaded (prefetch) and stored
+    add_quarters(c0v, w_iter); add_quarters(c1v, w_iter);
   }
-
-  // ---- 3. element -> node maps (needed by the hot blob) ----
-  const int na = npq + 2;      // + sentinel + trash records
-  std::vector<uint16_t> lptr(npq + 2, 0), lidx(std::max(1, nl)), sptr(npq + 2, 0), sidx(ng), xptr(npq + 2, 0), xidx;
+  for (size_t st = 0; st < bsched.size() / G; ++st) {
+    for (int l = 0; l < G; ++l) {
+      const uint64_t bd = bsched[st * G + l];
+      const unsigned bfl = static_cast<unsigned>(bd >> 32);
+      own[l] = static_cast<int>(bd & 0xFFFFu);
+      c0v[l] = (bfl & (kBschedRegParent | kBschedIdle)) ? -1 : static_cast<int>((bd >> 16) & 0xFFFFu);
+    }
+    add_quarters(own, 2.0 * w_iter); add_quarters(c0v, w_iter);
+  }
+  for (int b0 = 0; b0 < n; b0 += G) {                       // epilogue: per-bus loop, buses b0 + lane
+    for (int l = 0; l < G; ++l) own[l] = (b0 + l < n) ? node_of_bus[b0 + l] : -1;
+    add_quarters(own, 1.0);
+  }
   {
-    std::vector<std::vector<int>> ln(npq + 1), sn(npq + 1);
-    for (int l = 0; l < nl; ++l) ln[node_of_bus[net->load_bus[l]]].push_back(l);
-    for (int j = 0; j < ng; ++j) sn[node_of_bus[net->sgen_bus[j]]].push_back(j);
-    int a = 0, b = 0;
-    for (int i = 0; i <= npq; ++i) {
-      lptr[i] = static_cast<uint16_t>(a); sptr[i] = static_cast<uint16_t>(b);
-      xptr[i] = static_cast<uint16_t>(xidx.size());
-      for (int l : ln[i]) lidx[a++] = static_cast<uint16_t>(l);
-      const int bus = (i == npq) ? slack : order[i];
-      for (int j : sn[i]) {
-        sidx[b++] = static_cast<uint16_t>(j);
-        if (net->sgen_zone[j] == net->bus_zone[bus]) xidx.push_back(static_cast<uint16_t>(j));   // reference :238-244
-      }
+    std::vector<int> lf, lt;
+    for (size_t k = 0; k < y.from.size(); ++k) if (y.line[k]) { lf.push_back(node_of_bus[y.from[k]]); lt.push_back(node_of_bus[y.to[k]]); }
+    for (size_t k0 = 0; k0 < lf.size(); k0 += G) {
+      for (int l = 0; l < G; ++l) { own[l] = (k0 + l < lf.size()) ? lf[k0 + l] : -1; c0v[l] = (k0 + l < lt.size()) ? lt[k0 + l] : -1; }
+      add_quarters(own, 1.0); add_quarters(c0v, 1.0);
     }
-    lptr[npq + 1] = static_cast<uint16_t>(a); sptr[npq + 1] = static_cast<uint16_t>(b);
-    xptr[npq + 1] = static_cast<uint16_t>(xidx.size());
   }
-  // obs program (reference get_obs :232-274): per agent [P_zone | Q_zone | pv | q | vm_zone | va_zone | 0...].
-  // Hot copy: double offset of the source inside the env slab. Cold copy (get_obs_kernel): kind | node.
-  const int ssm = (cfg->state_space_mask & 31) ? (cfg->state_space_mask & 31) : 31;
+  // lab[base id] = label; sentinel / trash keep their ids
+  std::vector<int> lab(npq + 2), inv(npq + 2);
+  for (int i = 0; i < npq + 2; ++i) lab[i] = inv[i] = i;
+  auto extra = [&](const int* ids, int cnt) {               // extra wavefronts of one access: max multiplicity - 1
+    int c[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    int mx = 0;
+    for (int k = 0; k < cnt; ++k) mx = std::max(mx, ++c[ids[k] & 7]);
+    return std::max(0, mx - 1);
+  };
+  auto cost = [&]() {
+    double tot = 0.0;
+    int ids[8];
+    for (const Grp& g : groups) {
+      int cnt = 0;
+      for (int v : g.nodes) ids[cnt++] = lab[v];
+      tot += g.w * extra(ids, cnt);
+    }
+    // passes: label L is handled by lane L % G in round L / G; neighbours reached by pointer
+    for (int L0 = 0; L0 < npq; L0 += 8) {
+      int pa[8], k0[8], k1[8], np = 0, n0 = 0, n1 = 0;
+      auto push_unique = [](int* a, int& cnt, int v) { for (int k = 0; k < cnt; ++k) if (a[k] == v) return; a[cnt++] = v; };
+      for (int L = L0; L < std::min(npq, L0 + 8); ++L) {
+        const int i = inv[L];
+        push_unique(pa, np, parent[i] >= 0 ? lab[parent[i]] : npq);
+        push_unique(k0, n0, lab[kid0[i]]); push_unique(k1, n1, lab[kid1[i]]);
+      }
+      tot += w_iter * (extra(pa, np) + extra(k0, n0) + extra(k1, n1));
+    }
+    return tot;
+  };
+  const double cost0 = cost();
+  double cur = cost0, best = cur;
+  std::vector<int> best_lab = lab;
+  uint64_t rng = 0x9E3779B97F4A7C15ull;
+  auto rnd = [&]() { rng ^= rng << 13; rng ^= rng >> 7; rng ^= rng << 17; return rng; };
+  const int iters = std::min(400 * npq, 30000);
+  double T = std::max(1.0, 0.02 * cur);
+  const double cool = std::pow(1e-3, 1.0 / std::max(1, iters));
+  for (int it = 0; it < iters && best > 0.0; ++it, T *= cool) {
+    const int a = static_cast<int>(rnd() % npq), b = static_cast<int>(rnd() % npq);
+    if (a == b || ((lab[a] ^ lab[b]) & 7) == 0) continue;  // same residue: no effect on any group
+    std::swap(lab[a], lab[b]); inv[lab[a]] = a; inv[lab[b]] = b;
+    const double c2 = cost();
+    const double u = static_cast<double>(rnd() >> 11) * (1.0 / 9007199254740992.0);
+    if (c2 <= cur || u < std::exp((cur - c2) / T)) {
+      cur = c2;
+      if (cur < best) { best = cur; best_lab = lab; }
+    } else {
+      std::swap(lab[a], lab[b]); inv[lab[a]] = a; inv[lab[b]] = b;
+    }
+  }
+  lab = best_lab;
+  if (best < cost0) {
+    // apply: new id of base node i is lab[i]
+    std::vector<int> order2(npq), parent2(npq), nchild2(npq), k0b(npq), k1b(npq);
+    for (int i = 0; i < npq; ++i) {
+      const int L = lab[i];
+      order2[L] = order[i];
+      parent2[L] = parent[i] >= 0 ? lab[parent[i]] : -1;
+      nchild2[L] = nchild[i];
+      k0b[L] = lab[kid0[i]]; k1b[L] = lab[kid1[i]];
+    }
+    order = order2; parent = parent2; nchild = nchild2; kid0 = k0b; kid1 = k1b;
+    for (int i = 0; i < npq; ++i) node_of_bus[order[i]] = i;
+    auto map16 = [&](uint64_t v) { return static_cast<uint64_t>(lab[static_cast<int>(v & 0xFFFFu)]); };
+    for (uint64_t& ed : esched)
+      ed = (ed & 0xFFFF000000000000ull) | map16(ed) | (map16(ed >> 16) << 16) | (map16(ed >> 32) << 32);
+    for (uint64_t& bd : bsched)
+      bd = (bd & 0xFFFFFFFF00000000ull) | map16(bd) | (map16(bd >> 16) << 16);
+  }
+  if (getenv("MAPDN_DEBUG_SCHED"))
+    fprintf(stderr, "[relabel] weighted extra shared-memory wavefronts per env-step: %.1f -> %.1f (%d swaps tried)\n",
+            cost0, best, iters);
+}
+
+struct ElementMaps { std::vector<uint16_t> lptr, lidx, sptr, sidx, xptr, xidx; };   // node -> loads / sgens / sgens of the node's zone (CSR)
+
+// ---- 3. element -> node maps (needed by the hot blob) ----
+ElementMaps element_maps(const mapdn_net_desc& net, const Forest& f) {
+  const int npq = f.npq, nl = net.n_load, ng = net.n_sgen;
+  ElementMaps m;
+  m.lptr.assign(npq + 2, 0); m.lidx.resize(std::max(1, nl)); m.sptr.assign(npq + 2, 0); m.sidx.resize(ng); m.xptr.assign(npq + 2, 0);
+  std::vector<std::vector<int>> ln(npq + 1), sn(npq + 1);
+  for (int l = 0; l < nl; ++l) ln[f.node_of_bus[net.load_bus[l]]].push_back(l);
+  for (int j = 0; j < ng; ++j) sn[f.node_of_bus[net.sgen_bus[j]]].push_back(j);
+  int a = 0, b = 0;
+  for (int i = 0; i <= npq; ++i) {
+    m.lptr[i] = static_cast<uint16_t>(a); m.sptr[i] = static_cast<uint16_t>(b);
+    m.xptr[i] = static_cast<uint16_t>(m.xidx.size());
+    for (int l : ln[i]) m.lidx[a++] = static_cast<uint16_t>(l);
+    const int bus = (i == npq) ? f.slack : f.order[i];
+    for (int j : sn[i]) {
+      m.sidx[b++] = static_cast<uint16_t>(j);
+      if (net.sgen_zone[j] == net.bus_zone[bus]) m.xidx.push_back(static_cast<uint16_t>(j));   // reference :238-244
+    }
+  }
+  m.lptr[npq + 1] = static_cast<uint16_t>(a); m.sptr[npq + 1] = static_cast<uint16_t>(b);
+  m.xptr[npq + 1] = static_cast<uint16_t>(m.xidx.size());
+  return m;
+}
+
+// Slab offset (in doubles) of the sentinel record's UP.x: constant zero. The obs padding reads it.
+int zero_slot(int npq) { return 2 * (npq * kNodeArrays2 + A_UP); }
+
+struct ObsPrograms {
+  int obs_dim = 0, pvq_off2 = 0, scratch_off2 = 0;
+  std::vector<uint16_t> obs_off, obs_compact;          // hot copies: padded rows, rows without the padding
+  std::vector<unsigned> obs_src, state_src;            // cold copies: kind | node, kind | bus or sgen
+  std::vector<int> obs_xptr, obs_xidx;                 // sgens to add back per obs entry (CSR)
+  std::vector<int> agent_len, agent_off;               // compact rows: true length / offset of every agent's block
+};
+
+// obs program (reference get_obs :232-274): per agent [P_zone | Q_zone | pv | q | vm_zone | va_zone | 0...].
+// Hot copy: double offset of the source inside the env slab. Cold copy (get_obs_kernel): kind | node.
+mapdn_status obs_programs(const mapdn_net_desc& net, const Forest& f, int G, int state_space_mask, ObsPrograms& o) {
+  const int n = f.n, npq = f.npq, nl = net.n_load, ng = net.n_sgen;
+  const std::vector<int>& node_of_bus = f.node_of_bus;
+  const int ssm = (state_space_mask & 31) ? (state_space_mask & 31) : 31;
   const bool ss_dem = ssm & 1, ss_pv = ssm & 2, ss_q = ssm & 4, ss_vm = ssm & 8, ss_va = ssm & 16;
   int obs_dim = 0;
   std::vector<std::vector<int>> zb(ng);
   for (int a = 0; a < ng; ++a) {
-    for (int b = 0; b < n; ++b) if (net->bus_zone[b] == net->sgen_zone[a]) zb[a].push_back(b);
+    for (int b = 0; b < n; ++b) if (net.bus_zone[b] == net.sgen_zone[a]) zb[a].push_back(b);
     const int nz = static_cast<int>(zb[a].size());
     obs_dim = std::max(obs_dim, nz * (2 * ss_dem + ss_vm + ss_va) + ss_pv + ss_q);
   }
-  const int pvq_off2 = kNodeArrays2 * na, scratch_off2 = pvq_off2 + ng;
+  const int pvq_off2 = kNodeArrays2 * (npq + 2), scratch_off2 = pvq_off2 + ng;      // + sentinel + trash records
   if (2 * (scratch_off2 + (scratch_doubles_for(ng, nl, G, false) + 1) / 2) >= 65535)
-    return bail(fail(MAPDN_ERR_UNSUPPORTED, "network too large for 16-bit slab offsets"));
-  std::vector<uint16_t> obs_off(static_cast<size_t>(ng) * obs_dim);
-  std::vector<unsigned> obs_src(static_cast<size_t>(ng) * obs_dim, 0u);
-  std::vector<int> obs_xptr(static_cast<size_t>(ng) * obs_dim + 1, 0), obs_xidx;
-  std::vector<int> agent_len(ng, 0);
+    return fail(MAPDN_ERR_UNSUPPORTED, "network too large for 16-bit slab offsets");
+  o.obs_dim = obs_dim; o.pvq_off2 = pvq_off2; o.scratch_off2 = scratch_off2;
+  o.obs_off.resize(static_cast<size_t>(ng) * obs_dim);
+  o.obs_src.assign(static_cast<size_t>(ng) * obs_dim, 0u);
+  o.obs_xptr.assign(static_cast<size_t>(ng) * obs_dim + 1, 0);
+  o.agent_len.assign(ng, 0);
   auto src = [](ObsKind kind, int ix) { return (static_cast<unsigned>(kind) << 28) | static_cast<unsigned>(ix); };
   for (int a = 0; a < ng; ++a) {
     // entry list of this agent in the reference's order (:254-266), then zero padding (:270-274)
@@ -907,12 +968,12 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
     if (ss_q) ent.push_back({OBS_QSG, a});
     if (ss_vm) for (int b : zb[a]) ent.push_back({OBS_VM, b});
     if (ss_va) for (int b : zb[a]) ent.push_back({OBS_VA, b});
-    agent_len[a] = static_cast<int>(ent.size());
+    o.agent_len[a] = static_cast<int>(ent.size());
     for (int k = 0; k < obs_dim; ++k) {
       const size_t idx = static_cast<size_t>(a) * obs_dim + k;
-      obs_xptr[idx] = static_cast<int>(obs_xidx.size());
+      o.obs_xptr[idx] = static_cast<int>(o.obs_xidx.size());
       ObsKind kind = OBS_ZERO;
-      int ix = 0, off = 2 * (npq * kNodeArrays2 + A_UP);               // sentinel record's UP.x: constant zero
+      int ix = 0, off = zero_slot(npq);
       if (k < static_cast<int>(ent.size())) {
         kind = ent[k].first;
         const int t2 = ent[k].second;
@@ -920,147 +981,150 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
           ix = node_of_bus[t2];
           off = 2 * (node_of_bus[t2] * kNodeArrays2 + A_OP) + (kind == OBS_P ? 0 : 1);
           for (int j = 0; j < ng; ++j)
-            if (net->sgen_zone[j] == net->sgen_zone[a] && net->sgen_bus[j] == t2) obs_xidx.push_back(j);
+            if (net.sgen_zone[j] == net.sgen_zone[a] && net.sgen_bus[j] == t2) o.obs_xidx.push_back(j);
         } else if (kind == OBS_PV) { ix = t2; off = 2 * pvq_off2 + t2; }
         else if (kind == OBS_QSG) { ix = t2; off = 2 * pvq_off2 + ng + t2; }
         else { ix = node_of_bus[t2]; off = 2 * (node_of_bus[t2] * kNodeArrays2 + A_VV) + (kind == OBS_VM ? 0 : 1); }
       }
-      obs_src[idx] = src(kind, ix);
-      obs_off[idx] = static_cast<uint16_t>(off);
+      o.obs_src[idx] = src(kind, ix);
+      o.obs_off[idx] = static_cast<uint16_t>(off);
     }
   }
-  obs_xptr[static_cast<size_t>(ng) * obs_dim] = static_cast<int>(obs_xidx.size());
+  o.obs_xptr[static_cast<size_t>(ng) * obs_dim] = static_cast<int>(o.obs_xidx.size());
   // the same program without the padding: agent blocks back to back, the row rounded up to 4 entries (16-byte pieces of
   // fp32 rows) with reads of the zero slot
-  std::vector<uint16_t> obs_compact;
-  std::vector<int> agent_off(ng, 0);
+  o.agent_off.assign(ng, 0);
   for (int a = 0; a < ng; ++a) {
-    agent_off[a] = static_cast<int>(obs_compact.size());
-    for (int k = 0; k < agent_len[a]; ++k) obs_compact.push_back(obs_off[static_cast<size_t>(a) * obs_dim + k]);
+    o.agent_off[a] = static_cast<int>(o.obs_compact.size());
+    for (int k = 0; k < o.agent_len[a]; ++k) o.obs_compact.push_back(o.obs_off[static_cast<size_t>(a) * obs_dim + k]);
   }
-  while (obs_compact.size() % 4) obs_compact.push_back(static_cast<uint16_t>(2 * (npq * kNodeArrays2 + A_UP)));
+  while (o.obs_compact.size() % 4) o.obs_compact.push_back(static_cast<uint16_t>(zero_slot(npq)));
   // state program (reference get_state :213-230), bus-indexed
-  std::vector<unsigned> state_src;
+  std::vector<unsigned>& state_src = o.state_src;
   if (ss_dem) { for (int b = 0; b < n; ++b) state_src.push_back(src(OBS_PBUS, b)); for (int b = 0; b < n; ++b) state_src.push_back(src(OBS_QBUS, b)); }
   if (ss_pv) for (int j = 0; j < ng; ++j) state_src.push_back(src(OBS_PV, j));
   if (ss_q) for (int j = 0; j < ng; ++j) state_src.push_back(src(OBS_QSG, j));
   if (ss_vm) for (int b = 0; b < n; ++b) state_src.push_back(src(OBS_VM, b));
   if (ss_va) for (int b = 0; b < n; ++b) state_src.push_back(src(OBS_VA_DEG, b));
-  const int state_dim = static_cast<int>(state_src.size());
+  return MAPDN_OK;
+}
 
-  // ---- 3a. line-loss table + scaling ----
-  std::vector<double> lscale = vec_or(net->load_scaling, nl, 1.0), sscale = vec_or(net->sgen_scaling, ng, 1.0);
-  std::vector<uint16_t> line_nodes;
-  std::vector<double> line_c;
-  for (int k = 0; k < nbr; ++k) {
-    if (!br_line[k]) continue;
-    const double* y = &e->ybr[8 * static_cast<size_t>(k)];
-    line_nodes.push_back(static_cast<uint16_t>(node_of_bus[e->br_from[k]]));
-    line_nodes.push_back(static_cast<uint16_t>(node_of_bus[e->br_to[k]]));
-    // pl = Re(Sf + St) = Gff|Vf|^2 + Gtt|Vt|^2 + (Gft+Gtf) Re(Vf Vt*) + (Bft-Btf) Im(Vf Vt*)   [x baseMVA]
-    line_c.push_back(y[0] * net->base_mva); line_c.push_back(y[6] * net->base_mva);
-    line_c.push_back((y[2] + y[4]) * net->base_mva); line_c.push_back((y[3] - y[5]) * net->base_mva);
-  }
-  const int n_line = static_cast<int>(line_nodes.size() / 2);
-
-  // PQ-PQ Ybus pattern (CSR) for the dense fallback
-  std::vector<uint16_t> nbr_ptr(1, 0), nbr_idx;
+struct BranchTables {
+  int n_line = 0;
+  std::vector<uint16_t> line_nodes;          // [2 * n_line] from / to node; never empty, see below
+  std::vector<double> line_c;                // [4 * n_line] loss coefficients
+  std::vector<uint16_t> nbr_ptr, nbr_idx;    // meshed nets: CSR of the PQ-PQ Ybus pattern
   std::vector<double> nbr_y;
-  if (meshed) {
-    nbr_ptr.assign(npq + 1, 0);
-    for (int i = 0; i < npq; ++i) {
-      const int b = order[i];
-      for (int v : adj[b]) {
-        if (v == slack) continue;
-        double g, bb;
-        yoff(b, v, g, bb);
-        nbr_idx.push_back(static_cast<uint16_t>(node_of_bus[v])); nbr_y.push_back(g); nbr_y.push_back(bb);
-      }
-      nbr_ptr[i + 1] = static_cast<uint16_t>(nbr_idx.size());
-    }
-  }
-  // ---- 3b. hot static blob ----
-  HotLayout hl{};
-  int bytes_core = 0, bytes_full = 0;
-  {
-    int off = 0;
-    auto take = [&](size_t bytes) { int o = off; off += static_cast<int>((bytes + 15) / 16 * 16); return o; };
-    hl.yup = take(16 * npq); hl.ydn = take(16 * (npq + 1)); hl.yii = take(16 * npq);
-    hl.ndesc = take(8 * npq); hl.esched = take(8 * esched.size()); hl.bsched = take(8 * bsched.size());
-    hl.lptr = take(2 * lptr.size()); hl.lidx = take(2 * lidx.size());
-    hl.sptr = take(2 * sptr.size()); hl.sidx = take(2 * sidx.size());
-    hl.xptr = take(2 * xptr.size()); hl.xidx = take(2 * std::max<size_t>(1, xidx.size()));
-    hl.node_of_bus = take(2 * n);
-    hl.nbr_ptr = take(2 * nbr_ptr.size()); hl.nbr_idx = take(2 * std::max<size_t>(1, nbr_idx.size()));
-    hl.nbr_y = take(8 * std::max<size_t>(2, nbr_y.size()));
-    bytes_core = off;
-    // the once-per-step tables go last: the TMA copy either includes them (hl.bytes = bytes_full) or stops before them
-    if (line_nodes.empty()) { line_nodes.assign(2, 0); line_c.assign(4, 0.0); }
-    hl.ysl = take(16 * npq); hl.obs_off = take(2 * obs_off.size());
-    hl.line_nodes = take(2 * line_nodes.size()); hl.line_c = take(8 * line_c.size());
-    bytes_full = off;
-    hl.bytes = bytes_full; hl.tables_in_blob = 1;
-  }
-  std::vector<unsigned char> hot(bytes_full, 0);
-  std::vector<double> ysl_cold(2 * static_cast<size_t>(npq), 0.0);     // Y[i,slack]: cold table, non-zero for a few buses
-  std::vector<int> sl_node;
-  std::vector<double> sl_y;
-  {
-    double* yup = reinterpret_cast<double*>(hot.data() + hl.yup); double* ydn = reinterpret_cast<double*>(hot.data() + hl.ydn);
-    double* yii = reinterpret_cast<double*>(hot.data() + hl.yii);
-    double* ysl = ysl_cold.data();
-    uint64_t* ndesc = reinterpret_cast<uint64_t*>(hot.data() + hl.ndesc);
-    for (int i = 0; i < npq; ++i) {
-      const int b = order[i];
-      yii[2 * i] = e->ydiag[2 * b]; yii[2 * i + 1] = e->ydiag[2 * b + 1];
-      if (parent[i] >= 0) {
-        yoff(b, parent_bus[b], yup[2 * i], yup[2 * i + 1]);       // Y[i,parent]
-        yoff(parent_bus[b], b, ydn[2 * i], ydn[2 * i + 1]);       // Y[parent,i]
-      }
-      if (pairs.count({std::min(b, slack), std::max(b, slack)})) {
-        yoff(b, slack, ysl[2 * i], ysl[2 * i + 1]);               // Y[i,slack]
-        double g, bb;
-        yoff(slack, b, g, bb);                                     // Y[slack,i]
-        sl_node.push_back(i); sl_y.push_back(g); sl_y.push_back(bb);
-      }
-      // parent | child0 | child1 | number of further children (contiguous after child1); npq = zero slot
-      const uint64_t pa = parent[i] >= 0 ? static_cast<uint64_t>(parent[i]) : npq;   // roots: sentinel, Y = 0
-      const uint64_t c0 = static_cast<uint64_t>(kid0[i]), c1 = static_cast<uint64_t>(kid1[i]);   // npq = none
-      const uint64_t nx = nchild[i] > 2 ? nchild[i] - 2 : 0;
-      const uint64_t sl_adj = pairs.count({std::min(b, slack), std::max(b, slack)}) ? 1 : 0;
-      ndesc[i] = pa | (c0 << 16) | (c1 << 32) | (nx << 48) | (sl_adj << 63);
-    }
-    std::memcpy(hot.data() + hl.esched, esched.data(), 8 * esched.size());
-    std::memcpy(hot.data() + hl.bsched, bsched.data(), 8 * bsched.size());
-    std::memcpy(hot.data() + hl.lptr, lptr.data(), 2 * lptr.size());
-    if (nl) std::memcpy(hot.data() + hl.lidx, lidx.data(), 2 * static_cast<size_t>(nl));
-    std::memcpy(hot.data() + hl.sptr, sptr.data(), 2 * sptr.size());
-    std::memcpy(hot.data() + hl.sidx, sidx.data(), 2 * sidx.size());
-    std::memcpy(hot.data() + hl.xptr, xptr.data(), 2 * xptr.size());
-    if (!xidx.empty()) std::memcpy(hot.data() + hl.xidx, xidx.data(), 2 * xidx.size());
-    std::memcpy(hot.data() + hl.ysl, ysl_cold.data(), 8 * ysl_cold.size());
-    std::memcpy(hot.data() + hl.obs_off, obs_off.data(), 2 * obs_off.size());
-    std::memcpy(hot.data() + hl.line_nodes, line_nodes.data(), 2 * line_nodes.size());
-    std::memcpy(hot.data() + hl.line_c, line_c.data(), 8 * line_c.size());
-    uint16_t* nob = reinterpret_cast<uint16_t*>(hot.data() + hl.node_of_bus);
-    for (int b = 0; b < n; ++b) nob[b] = static_cast<uint16_t>(node_of_bus[b]);
-    std::memcpy(hot.data() + hl.nbr_ptr, nbr_ptr.data(), 2 * nbr_ptr.size());
-    if (!nbr_idx.empty()) {
-      std::memcpy(hot.data() + hl.nbr_idx, nbr_idx.data(), 2 * nbr_idx.size());
-      std::memcpy(hot.data() + hl.nbr_y, nbr_y.data(), 8 * nbr_y.size());
-    }
-  }
+};
 
-  // ---- 5. launch geometry ----
-  cudaDeviceProp dp{};
-  TRY_CUDA(cudaGetDeviceProperties(&dp, device));
-  const size_t max_smem = dp.sharedMemPerBlockOptin;
-  // envs per CTA: sub-warp groups pack 32/G envs into each of 1..4 solver warps; multi-warp groups (G = 64 / 128)
-  // put 1..4 envs of G threads in a CTA. Fewer envs per CTA when that spreads the batch over all SMs.
+// ---- 3a. line-loss table, and the PQ-PQ Ybus pattern (CSR) for the dense fallback ----
+BranchTables branch_tables(const Ybus& y, const Forest& f, double base_mva) {
+  BranchTables t;
+  for (size_t k = 0; k < y.from.size(); ++k) {
+    if (!y.line[k]) continue;
+    const double* yk = &y.ybr[8 * k];
+    t.line_nodes.push_back(static_cast<uint16_t>(f.node_of_bus[y.from[k]]));
+    t.line_nodes.push_back(static_cast<uint16_t>(f.node_of_bus[y.to[k]]));
+    // pl = Re(Sf + St) = Gff|Vf|^2 + Gtt|Vt|^2 + (Gft+Gtf) Re(Vf Vt*) + (Bft-Btf) Im(Vf Vt*)   [x baseMVA]
+    t.line_c.push_back(yk[0] * base_mva); t.line_c.push_back(yk[6] * base_mva);
+    t.line_c.push_back((yk[2] + yk[4]) * base_mva); t.line_c.push_back((yk[3] - yk[5]) * base_mva);
+  }
+  t.n_line = static_cast<int>(t.line_nodes.size() / 2);
+  // a net without lines keeps one all-zero entry in the hot blob and in the cold copies: n_line stays 0
+  if (t.line_nodes.empty()) { t.line_nodes.assign(2, 0); t.line_c.assign(4, 0.0); }
+  t.nbr_ptr.assign(1, 0);
+  if (f.meshed) {
+    t.nbr_ptr.assign(f.npq + 1, 0);
+    for (int i = 0; i < f.npq; ++i) {
+      const int b = f.order[i];
+      for (int v : f.adj[b]) {
+        if (v == f.slack) continue;
+        double g, bb;
+        yoff(f.pairs, b, v, g, bb);
+        t.nbr_idx.push_back(static_cast<uint16_t>(f.node_of_bus[v])); t.nbr_y.push_back(g); t.nbr_y.push_back(bb);
+      }
+      t.nbr_ptr[i + 1] = static_cast<uint16_t>(t.nbr_idx.size());
+    }
+  }
+  return t;
+}
+
+struct HotBlob {
+  HotLayout hl{};                            // offsets only: bytes / tables_in_blob follow from the launch geometry
+  std::vector<unsigned char> blob;           // bytes_full bytes
+  int bytes_core = 0, bytes_full = 0;        // without / with the once-per-step tables
+  std::vector<double> ysl_cold;              // Y[i,slack]: cold table, non-zero for a few buses
+  std::vector<int> sl_node;                  // the slack-adjacent nodes and their Y[slack,i]
+  std::vector<double> sl_y;
+};
+
+// Appends a table to the blob at the next 16-byte boundary and returns its byte offset. The slot holds at least min_count
+// entries (zeros beyond the table's own): the kernel addresses some tables that can be empty.
+template <class T>
+int blob_put(std::vector<unsigned char>& blob, const std::vector<T>& v, size_t min_count = 0) {
+  const size_t off = blob.size();
+  blob.resize(off + (std::max(v.size(), min_count) * sizeof(T) + 15) / 16 * 16, 0);
+  if (!v.empty()) std::memcpy(blob.data() + off, v.data(), v.size() * sizeof(T));
+  return static_cast<int>(off);
+}
+
+// ---- 3b. hot static blob ----
+HotBlob build_hot_blob(const Ybus& y, const Forest& f, const Sweeps& s, const ElementMaps& m, const ObsPrograms& o,
+                       const BranchTables& t) {
+  const int npq = f.npq, slack = f.slack;
+  HotBlob h;
+  std::vector<double> yup(2 * static_cast<size_t>(npq), 0.0), ydn(2 * static_cast<size_t>(npq + 1), 0.0), yii(2 * static_cast<size_t>(npq));
+  std::vector<uint64_t> ndesc(npq);
+  h.ysl_cold.assign(2 * static_cast<size_t>(npq), 0.0);
+  double* ysl = h.ysl_cold.data();
+  for (int i = 0; i < npq; ++i) {
+    const int b = f.order[i];
+    yii[2 * i] = y.ydiag[2 * b]; yii[2 * i + 1] = y.ydiag[2 * b + 1];
+    if (f.parent[i] >= 0) {
+      yoff(f.pairs, b, f.parent_bus[b], yup[2 * i], yup[2 * i + 1]);       // Y[i,parent]
+      yoff(f.pairs, f.parent_bus[b], b, ydn[2 * i], ydn[2 * i + 1]);       // Y[parent,i]
+    }
+    const uint64_t sl_adj = f.pairs.count({std::min(b, slack), std::max(b, slack)}) ? 1 : 0;
+    if (sl_adj) {
+      yoff(f.pairs, b, slack, ysl[2 * i], ysl[2 * i + 1]);               // Y[i,slack]
+      double g, bb;
+      yoff(f.pairs, slack, b, g, bb);                                    // Y[slack,i]
+      h.sl_node.push_back(i); h.sl_y.push_back(g); h.sl_y.push_back(bb);
+    }
+    // parent | child0 | child1 | number of further children (contiguous after child1); npq = zero slot
+    const uint64_t pa = f.parent[i] >= 0 ? static_cast<uint64_t>(f.parent[i]) : npq;   // roots: sentinel, Y = 0
+    const uint64_t c0 = static_cast<uint64_t>(f.kid0[i]), c1 = static_cast<uint64_t>(f.kid1[i]);   // npq = none
+    const uint64_t nx = f.nchild[i] > 2 ? f.nchild[i] - 2 : 0;
+    ndesc[i] = pa | (c0 << 16) | (c1 << 32) | (nx << 48) | (sl_adj << 63);
+  }
+  const std::vector<uint16_t> nob(f.node_of_bus.begin(), f.node_of_bus.end());
+  HotLayout& hl = h.hl;
+  hl.yup = blob_put(h.blob, yup); hl.ydn = blob_put(h.blob, ydn); hl.yii = blob_put(h.blob, yii);
+  hl.ndesc = blob_put(h.blob, ndesc); hl.esched = blob_put(h.blob, s.esched); hl.bsched = blob_put(h.blob, s.bsched);
+  hl.lptr = blob_put(h.blob, m.lptr); hl.lidx = blob_put(h.blob, m.lidx);
+  hl.sptr = blob_put(h.blob, m.sptr); hl.sidx = blob_put(h.blob, m.sidx);
+  hl.xptr = blob_put(h.blob, m.xptr); hl.xidx = blob_put(h.blob, m.xidx, 1);
+  hl.node_of_bus = blob_put(h.blob, nob);
+  hl.nbr_ptr = blob_put(h.blob, t.nbr_ptr); hl.nbr_idx = blob_put(h.blob, t.nbr_idx, 1); hl.nbr_y = blob_put(h.blob, t.nbr_y, 2);
+  h.bytes_core = static_cast<int>(h.blob.size());
+  // the once-per-step tables go last: the TMA copy either includes them (hl.bytes = bytes_full) or stops before them
+  hl.ysl = blob_put(h.blob, h.ysl_cold); hl.obs_off = blob_put(h.blob, o.obs_off);
+  hl.line_nodes = blob_put(h.blob, t.line_nodes); hl.line_c = blob_put(h.blob, t.line_c);
+  h.bytes_full = static_cast<int>(h.blob.size());
+  return h;
+}
+
+struct Geometry {
+  bool cold_tables = false, stage_rec = false;   // the two ways to buy shared memory, see below
+  int stride2 = 0, epb = 0, smem = 0, helper_threads = 32;
+};
+
+// ---- 5. launch geometry ----
+// envs per CTA: sub-warp groups pack 32/G envs into each of 1..4 solver warps; multi-warp groups (G = 64 / 128)
+// put 1..4 envs of G threads in a CTA. Fewer envs per CTA when that spreads the batch over all SMs.
+mapdn_status plan_geometry(int npq, int ng, int nl, int G, int batch, int bytes_core, int bytes_full, size_t max_smem,
+                           int n_sm, Geometry& geo) {
   const int unit = (G <= 32) ? 32 / G : 1;               // envs added per step of the search
-  const int n_sm = dp.multiProcessorCount;
-  int stride2 = 0, epb = 0;
-  bool stage_rec = false;
   // Two ways to buy shared memory when it limits the envs per SM, both with a price: (a) the four
   // once-per-step tables (Y[i,slack], obs program, line tables) stay in global memory instead of the staged blob - their
   // first touch after an L2 flush is an HBM round trip at the start of the epilogue, softened by an L2 prefetch at kernel
@@ -1083,7 +1147,7 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
     // SMs exactly (case33 x 4096 on 132 SMs: 128 CTAs of 32 envs). Many-round batches keep several small CTAs per SM.
     auto fits = [&](int c) { return smem_with(cold, pl.st2, c) <= max_smem && c * G <= (G <= 32 ? 256 : 512); };
     for (int r = 1; r <= 3; ++r) {
-      int c = (cfg->batch + n_sm * r - 1) / (n_sm * r);
+      int c = (batch + n_sm * r - 1) / (n_sm * r);
       c = (c + unit - 1) / unit * unit;
       if (fits(c)) { c_epb = std::max(c_epb, c); break; }
     }
@@ -1092,229 +1156,305 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
     while (c_epb > unit && (smem_with(cold, pl.st2, c_epb) > max_smem || c_epb * G > (G <= 32 ? 256 : 512))) c_epb -= unit;
     pl.epb = c_epb;
     pl.ok = smem_with(cold, pl.st2, c_epb) <= max_smem;
-    pl.rounds = (cfg->batch + static_cast<long long>(c_epb) * n_sm - 1) / (static_cast<long long>(c_epb) * n_sm);
+    pl.rounds = (batch + static_cast<long long>(c_epb) * n_sm - 1) / (static_cast<long long>(c_epb) * n_sm);
     return pl;
   };
-  bool cold_tables = false;
-  {
-    const Plan plans[4] = {make_plan(false, false), make_plan(false, true), make_plan(true, false), make_plan(true, true)};   // cheapest first
-    const Plan* best = nullptr;
-    for (const Plan& pl : plans) if (pl.ok && (!best || pl.rounds < best->rounds)) best = &pl;
-    if (const char* ov = getenv("MAPDN_PLAN")) {             // tuning override: 0..3 = index into the list above
-      const int k = atoi(ov);
-      if (k >= 0 && k < 4 && plans[k].ok) best = &plans[k];
-    }
-    if (best) { stride2 = best->st2; epb = best->epb; stage_rec = best->rec; cold_tables = best->cold; }
+  const Plan plans[4] = {make_plan(false, false), make_plan(false, true), make_plan(true, false), make_plan(true, true)};   // cheapest first
+  const Plan* best = nullptr;
+  for (const Plan& pl : plans) if (pl.ok && (!best || pl.rounds < best->rounds)) best = &pl;
+  if (const char* ov = getenv("MAPDN_PLAN")) {             // tuning override: 0..3 = index into the list above
+    const int k = atoi(ov);
+    if (k >= 0 && k < 4 && plans[k].ok) best = &plans[k];
   }
-  hl.tables_in_blob = cold_tables ? 0 : 1;
-  hl.bytes = cold_tables ? bytes_core : bytes_full;
-  auto smem_for = [&](int c) { return smem_with(cold_tables, stride2, c); };
-  if (epb == 0 || smem_for(epb) > max_smem)
-    return bail(fail(MAPDN_ERR_UNSUPPORTED, "network too large for the shared-memory resident solver (" +
-                                                std::to_string(smem_for(std::max(epb, unit))) + " B needed)"));
-  e->dense = meshed;
-  e->G = G; e->threads = epb * G; e->epb = epb; e->smem = static_cast<int>(smem_for(epb));
-  {   // helper warps (next profile rows + noise, concurrent with the Newton iteration): one per 256 Box-Muller pairs of a
-      // CTA round, at most 4 -- a single warp can be the critical path of case322
-    const int n_pair = (ng + 2 * nl + 1) / 2;
-    e->helper_threads = 32 * std::min(4, std::max(1, (epb * n_pair + kHelperPairsPerWarp - 1) / kHelperPairsPerWarp));
+  if (best) { geo.stride2 = best->st2; geo.epb = best->epb; geo.stage_rec = best->rec; geo.cold_tables = best->cold; }
+  auto smem_for = [&](int c) { return smem_with(geo.cold_tables, geo.stride2, c); };
+  if (geo.epb == 0 || smem_for(geo.epb) > max_smem)
+    return fail(MAPDN_ERR_UNSUPPORTED, "network too large for the shared-memory resident solver (" +
+                                           std::to_string(smem_for(std::max(geo.epb, unit))) + " B needed)");
+  geo.smem = static_cast<int>(smem_for(geo.epb));
+  // helper warps (next profile rows + noise, concurrent with the Newton iteration): one per 256 Box-Muller pairs of a
+  // CTA round, at most 4 -- a single warp can be the critical path of case322
+  const int n_pair = (ng + 2 * nl + 1) / 2;
+  geo.helper_threads = 32 * std::min(4, std::max(1, (geo.epb * n_pair + kHelperPairsPerWarp - 1) / kHelperPairsPerWarp));
+  if (const char* ov = getenv("MAPDN_HELPERS")) geo.helper_threads = 32 * std::min(4, std::max(1, atoi(ov)));   // tuning override
+  return MAPDN_OK;
+}
+
+// The flat start of the first Newton iteration: every PQ bus at vm_init, angle 0; the slack at vm0, va0 = e0 + j f0
+struct FlatStart { double vm_init, vm0, va0, e0, f0; };
+
+FlatStart flat_start(const mapdn_net_desc& net) {
+  FlatStart v{};
+  v.vm_init = (net.vm_init > 0) ? net.vm_init : net.slack_vm;
+  v.vm0 = net.slack_vm; v.va0 = net.slack_va_deg * (3.14159265358979323846 / 180.0);
+  v.e0 = v.vm0 * std::cos(v.va0); v.f0 = v.vm0 * std::sin(v.va0);
+  return v;
+}
+
+// The first Newton iteration starts from the flat start, where S_calc and the Jacobian depend on the network only:
+// factorise J(V0) once, leaf -> root on the elimination forest, with the formulas of the kernel's edge / mismatch pass
+// and elimination step (env_kernel.cuh: nr_solve). Per node six double2: S_calc = (P, Q); M = D'^-1 J[i,parent] rows
+// 0 / 1 (what the back sweep multiplies dx_parent with); D'^-1 rows 0 / 1; J[parent,i] = (a, b).
+std::vector<double> first_iteration_factors(const Forest& f, const HotBlob& hot, const FlatStart& v0) {
+  const int npq = f.npq;
+  std::vector<double> ft(static_cast<size_t>(12) * std::max(1, npq), 0.0);
+  if (f.meshed) return ft;
+  const double* yup = reinterpret_cast<const double*>(hot.blob.data() + hot.hl.yup);
+  const double* ydn = reinterpret_cast<const double*>(hot.blob.data() + hot.hl.ydn);
+  const double* yii = reinterpret_cast<const double*>(hot.blob.data() + hot.hl.yii);
+  const std::vector<double>& ysl_cold = hot.ysl_cold;
+  // children in a labelling-independent order (first child, second child, then the contiguous extras): the node
+  // relabelling of section 2b must not change a single bit of the results
+  std::vector<std::vector<int>> kids(npq);
+  for (int i = 0; i < npq; ++i) {
+    if (f.kid0[i] != npq) kids[i].push_back(f.kid0[i]);
+    if (f.kid1[i] != npq) kids[i].push_back(f.kid1[i]);
+    for (int c = 2; c < f.nchild[i]; ++c) kids[i].push_back(f.kid1[i] + c - 1);      // extras follow child 1 contiguously
   }
-  if (const char* ov = getenv("MAPDN_HELPERS")) e->helper_threads = 32 * std::min(4, std::max(1, atoi(ov)));   // tuning override
-  for (int mode = 0; mode < 7; ++mode) {      // 4: MODE_STEP with tester records; 5, 6: with history, without / with records
-    KernelFn fn = (mode < 4) ? kernel_for(G, mode, meshed) : kernel_for(G, MODE_STEP, meshed, mode != 5, mode > 4);
+  std::vector<int> topo;                               // parents before children
+  for (int i = 0; i < npq; ++i) if (f.parent[i] < 0) topo.push_back(i);
+  for (size_t qh = 0; qh < topo.size(); ++qh) for (int c : kids[topo[qh]]) topo.push_back(c);
+  const double vi_x = v0.vm_init, vi_y = 0.0;            // every PQ bus
+  std::vector<double> upx(npq), upy(npq), dnx(npq), dny(npq), d01x(npq), d01y(npq), d23x(npq), d23y(npq);
+  std::vector<double> s00(npq, 0.0), s01(npq, 0.0), s10(npq, 0.0), s11(npq, 0.0);     // Schur update a bus hands to its parent
+  for (int i = 0; i < npq; ++i) {                      // edge terms of (i, parent); roots: Y = 0
+    const double vp_x = v0.vm_init, vp_y = 0.0;
+    const double cc = vi_x * vp_x + vi_y * vp_y, ss = vi_y * vp_x - vi_x * vp_y;
+    upx[i] = yup[2 * i] * ss - yup[2 * i + 1] * cc; upy[i] = yup[2 * i] * cc + yup[2 * i + 1] * ss;
+    dnx[i] = -ydn[2 * i] * ss - ydn[2 * i + 1] * cc; dny[i] = ydn[2 * i] * cc - ydn[2 * i + 1] * ss;
+  }
+  for (int i = 0; i < npq; ++i) {                      // S_calc and the diagonal blocks
+    const double cs0 = vi_x * v0.e0 + vi_y * v0.f0, sn0 = vi_y * v0.e0 - vi_x * v0.f0;
+    double sa = ysl_cold[2 * i] * sn0 - ysl_cold[2 * i + 1] * cs0 + upx[i];
+    double sb = ysl_cold[2 * i] * cs0 + ysl_cold[2 * i + 1] * sn0 + upy[i];
+    for (int c : kids[i]) { sa += dnx[c]; sb += dny[c]; }
+    const double vv = vi_x * vi_x + vi_y * vi_y;
+    const double gv = yii[2 * i] * vv, bv = yii[2 * i + 1] * vv;
+    const double Pc = gv + sb, Qc = sa - bv;
+    ft[12 * i + 0] = Pc; ft[12 * i + 1] = Qc;
+    d01x[i] = -Qc - bv; d01y[i] = Pc + gv; d23x[i] = Pc - gv; d23y[i] = Qc - bv;
+  }
+  for (size_t k = topo.size(); k-- > 0;) {              // children before parents
+    const int i = topo[k];
+    for (int c : kids[i]) { d01x[i] -= s00[c]; d01y[i] -= s01[c]; d23x[i] -= s10[c]; d23y[i] -= s11[c]; }
+    const double idet = 1.0 / (d01x[i] * d23y[i] - d01y[i] * d23x[i]);
+    const double ux = upx[i], uy = upy[i], dx = dnx[i], dy = dny[i];
+    const double ma00 = d23y[i] * ux + d01y[i] * uy, ma01 = d23y[i] * uy - d01y[i] * ux;      // adj(D') J[i,parent]
+    const double ma10 = -d23x[i] * ux - d01x[i] * uy, ma11 = d01x[i] * ux - d23x[i] * uy;
+    ft[12 * i + 2] = ma00 * idet; ft[12 * i + 3] = ma01 * idet; ft[12 * i + 4] = ma10 * idet; ft[12 * i + 5] = ma11 * idet;
+    ft[12 * i + 6] = d23y[i] * idet; ft[12 * i + 7] = -d01y[i] * idet;                         // D'^-1
+    ft[12 * i + 8] = -d23x[i] * idet; ft[12 * i + 9] = d01x[i] * idet;
+    ft[12 * i + 10] = dx; ft[12 * i + 11] = dy;
+    s00[i] = (dx * ma00 + dy * ma10) * idet; s01[i] = (dx * ma01 + dy * ma11) * idet;         // J[parent,i] D'^-1 J[i,parent]
+    s10[i] = (dx * ma10 - dy * ma00) * idet; s11[i] = (dx * ma11 - dy * ma01) * idet;
+  }
+  return ft;
+}
+
+// The shared-memory attribute of the seven kernel instantiations the handle launches, and the persistent grid of the four
+// step variants (needs G, threads, helper_threads, smem and dense of the handle)
+mapdn_status size_kernels(mapdn_env* e, const cudaDeviceProp& dp) {
+  struct Variant { int mode; bool record, hist; };
+  const Variant variants[7] = {{MODE_STEP, false, false}, {MODE_STEP, true, false}, {MODE_STEP, false, true}, {MODE_STEP, true, true},
+                               {MODE_SOLVE, false, false}, {MODE_RESET, false, false}, {MODE_DROOP, false, false}};
+  for (const Variant& v : variants) {       // the plain step first: it bounds the grids of the other three
+    KernelFn fn = kernel_for(e->G, v.mode, e->dense, v.record, v.hist);
     // the attribute belongs to the function, not to the handle: always allow the device maximum, so that creating a
     // second handle with a smaller footprint cannot break the launches of the first
     cudaFuncAttributes fa{};
-    TRY_CUDA(cudaFuncGetAttributes(&fa, reinterpret_cast<const void*>(fn)));
-    const int dyn_max = static_cast<int>(max_smem - fa.sharedSizeBytes);        // opt-in limit minus the static part
-    if (e->smem > dyn_max)
-      return bail(fail(MAPDN_ERR_UNSUPPORTED, "network too large for the shared-memory resident solver"));
-    TRY_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn_max));
-  }
-  {
+    MAPDN_CUDA(cudaFuncGetAttributes(&fa, reinterpret_cast<const void*>(fn)));
+    const int dyn_max = static_cast<int>(dp.sharedMemPerBlockOptin - fa.sharedSizeBytes);        // opt-in limit minus the static part
+    if (e->smem > dyn_max) return fail(MAPDN_ERR_UNSUPPORTED, "network too large for the shared-memory resident solver");
+    MAPDN_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn_max));
+    if (v.mode != MODE_STEP) continue;
     int per_sm = 0;
-    TRY_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel_for(G, MODE_STEP, meshed), e->threads + e->helper_threads, e->smem));
-    e->max_blocks = std::max(1, per_sm) * dp.multiProcessorCount;
-    if (meshed) e->max_blocks = std::min(e->max_blocks, 2 * dp.multiProcessorCount);   // bounds the dense workspace
-    // the record instantiation holds more registers: its persistent grid is sized by its own occupancy (never larger)
-    TRY_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel_for(G, MODE_STEP, meshed, true), e->threads + e->helper_threads, e->smem));
-    e->max_blocks_record = std::min(e->max_blocks, std::max(1, per_sm) * dp.multiProcessorCount);
-    TRY_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel_for(G, MODE_STEP, meshed, false, true), e->threads + e->helper_threads, e->smem));
-    e->max_blocks_hist = std::min(e->max_blocks, std::max(1, per_sm) * dp.multiProcessorCount);
-    TRY_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel_for(G, MODE_STEP, meshed, true, true), e->threads + e->helper_threads, e->smem));
-    e->max_blocks_hist_record = std::min(e->max_blocks, std::max(1, per_sm) * dp.multiProcessorCount);
+    MAPDN_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, e->threads + e->helper_threads, e->smem));
+    int blocks = std::max(1, per_sm) * dp.multiProcessorCount;
+    if (e->dense) blocks = std::min(blocks, 2 * dp.multiProcessorCount);   // bounds the dense workspace
+    // the record and history instantiations hold more registers: each persistent grid is sized by its own occupancy
+    // (never larger than the plain step's)
+    if (v.record || v.hist) blocks = std::min(blocks, e->max_blocks_step[0][0]);
+    e->max_blocks_step[v.hist][v.record] = blocks;
   }
+  return MAPDN_OK;
+}
 
-  // ---- 6. upload + env state ----
+// ---- 6. upload + env state ----
+// Fills e->base from the plan, uploads every table and allocates the env state. Needs the handle's launch geometry and
+// the grid of the plain step (size_kernels): a meshed net's dense workspace has one slice per resident env group.
+mapdn_status upload_plan(mapdn_env* e, const mapdn_net_desc& net, const mapdn_profile_desc* prof, const Ybus& y,
+                         const Forest& f, const Sweeps& s, const ObsPrograms& o, const BranchTables& t, const HotBlob& hot,
+                         const Geometry& geo, const FlatStart& v0, const std::vector<double>& ft) {
+  const mapdn_cfg& cfg = e->cfg;
+  const int n = f.n, npq = f.npq, nl = net.n_load, ng = net.n_sgen, slack = f.slack;
   Params& P = e->base;
-  P.n_bus = n; P.npq = npq; P.n_load = nl; P.n_sgen = ng; P.n_line = n_line; P.n_lev = n_lev;
-  P.obs_dim = obs_dim; P.state_dim = state_dim; P.n_slack_adj = static_cast<int>(sl_node.size());
-  P.n_esteps = n_esteps; P.n_bsteps = n_bsteps; P.has_extra_children = max_children > 2;
-  P.n_wide_e = std::min(n_wide_e, n_esteps); P.n_narrow_b = std::min(n_narrow_b, n_bsteps);
+  P.n_bus = n; P.npq = npq; P.n_load = nl; P.n_sgen = ng; P.n_line = t.n_line; P.n_lev = f.n_lev;
+  P.obs_dim = o.obs_dim; P.state_dim = static_cast<int>(o.state_src.size()); P.n_slack_adj = static_cast<int>(hot.sl_node.size());
+  P.n_esteps = s.n_esteps(); P.n_bsteps = s.n_bsteps(); P.has_extra_children = f.max_children > 2;
+  P.n_wide_e = std::min(s.n_wide_e, P.n_esteps); P.n_narrow_b = std::min(s.n_narrow_b, P.n_bsteps);
   P.slack_bus = slack;
-  P.nb = cfg->batch; P.env_stride2 = stride2; P.pvq_off2 = pvq_off2; P.scratch_off2 = scratch_off2; P.hot_layout = hl;
-  P.helper_off = hl.bytes + e->epb * stride2 * 16;
-  P.stage_in_records = stage_rec ? 1 : 0;
+  P.nb = cfg.batch; P.env_stride2 = geo.stride2; P.pvq_off2 = o.pvq_off2; P.scratch_off2 = o.scratch_off2;
+  P.hot_layout = hot.hl;
+  P.hot_layout.tables_in_blob = geo.cold_tables ? 0 : 1;
+  P.hot_layout.bytes = geo.cold_tables ? hot.bytes_core : hot.bytes_full;
+  P.helper_off = P.hot_layout.bytes + e->epb * geo.stride2 * 16;
+  P.stage_in_records = geo.stage_rec ? 1 : 0;
   P.obs_skip_off = -1;
   P.history = 1;
-  e->obs_zero_off = 2 * (npq * kNodeArrays2 + A_UP);
-  TRY(dev_upload(e, obs_compact, &P.obs_compact_prog));
+  e->obs_zero_off = zero_slot(npq);
+  MAPDN_TRY(dev_upload(e, o.obs_compact, &P.obs_compact_prog));
   P.obs_compact_len = 0;
-  e->agent_len = agent_len; e->agent_off = agent_off; e->compact_row = static_cast<int>(obs_compact.size());
+  e->agent_len = o.agent_len; e->agent_off = o.agent_off; e->compact_row = static_cast<int>(o.obs_compact.size());
   {   // bus shunts by node (res_bus p/q carry the shunt power, pandapower _get_shunt_results)
     std::vector<double> sh_g(npq + 1), sh_b(npq + 1);
     bool any = false;
     for (int i = 0; i <= npq; ++i) {
-      const int b = (i == npq) ? slack : order[i];
-      sh_g[i] = gs[b]; sh_b[i] = bs[b];
-      any = any || gs[b] != 0.0 || bs[b] != 0.0;
+      const int b = (i == npq) ? slack : f.order[i];
+      sh_g[i] = y.gs[b]; sh_b[i] = y.bs[b];
+      any = any || y.gs[b] != 0.0 || y.bs[b] != 0.0;
     }
     P.has_shunt = any;
-    TRY(dev_upload(e, sh_g, &P.sh_g)); TRY(dev_upload(e, sh_b, &P.sh_b));
+    MAPDN_TRY(dev_upload(e, sh_g, &P.sh_g)); MAPDN_TRY(dev_upload(e, sh_b, &P.sh_b));
   }
-  std::vector<int> bus_of_node(order.begin(), order.end());
-  TRY(dev_upload(e, hot, &P.hot));
-  TRY(dev_upload(e, bus_of_node, &P.bus_of_node));
-  TRY(dev_upload(e, lscale, &P.lscale)); TRY(dev_upload(e, sscale, &P.sscale));
-  TRY(dev_upload(e, sl_node, &P.sl_node)); TRY(dev_upload(e, sl_y, &P.sl_y));
+  MAPDN_TRY(dev_upload(e, hot.blob, &P.hot));
+  MAPDN_TRY(dev_upload(e, f.order, &P.bus_of_node));
+  MAPDN_TRY(dev_upload(e, vec_or(net.load_scaling, nl, 1.0), &P.lscale));
+  MAPDN_TRY(dev_upload(e, vec_or(net.sgen_scaling, ng, 1.0), &P.sscale));
+  MAPDN_TRY(dev_upload(e, hot.sl_node, &P.sl_node)); MAPDN_TRY(dev_upload(e, hot.sl_y, &P.sl_y));
   {
-    const double* d_ysl = nullptr;
-    TRY(dev_upload(e, ysl_cold, &d_ysl));
+    const double *d_ysl = nullptr, *d_ft = nullptr;
+    MAPDN_TRY(dev_upload(e, hot.ysl_cold, &d_ysl));
     P.ysl = reinterpret_cast<const double2*>(d_ysl);
-    TRY(dev_upload(e, obs_off, &P.obs_off)); TRY(dev_upload(e, line_nodes, &P.line_nodes)); TRY(dev_upload(e, line_c, &P.line_c));
+    MAPDN_TRY(dev_upload(e, ft, &d_ft));
+    P.first_tab = reinterpret_cast<const double2*>(d_ft);
   }
+  MAPDN_TRY(dev_upload(e, o.obs_off, &P.obs_off));
+  MAPDN_TRY(dev_upload(e, t.line_nodes, &P.line_nodes)); MAPDN_TRY(dev_upload(e, t.line_c, &P.line_c));
   {
     std::vector<int> sgen_node(ng);
-    for (int j = 0; j < ng; ++j) sgen_node[j] = node_of_bus[net->sgen_bus[j]];
-    TRY(dev_upload(e, sgen_node, &P.sgen_node));
+    for (int j = 0; j < ng; ++j) sgen_node[j] = f.node_of_bus[net.sgen_bus[j]];
+    MAPDN_TRY(dev_upload(e, sgen_node, &P.sgen_node));
   }
-  TRY(dev_upload(e, state_src, &P.state_src)); TRY(dev_upload(e, obs_src, &P.obs_src)); TRY(dev_upload(e, obs_xptr, &P.obs_xptr)); TRY(dev_upload(e, obs_xidx, &P.obs_xidx));
-  const size_t B = static_cast<size_t>(cfg->batch);
+  MAPDN_TRY(dev_upload(e, o.state_src, &P.state_src)); MAPDN_TRY(dev_upload(e, o.obs_src, &P.obs_src));
+  MAPDN_TRY(dev_upload(e, o.obs_xptr, &P.obs_xptr)); MAPDN_TRY(dev_upload(e, o.obs_xidx, &P.obs_xidx));
+  const size_t B = static_cast<size_t>(cfg.batch);
   if (prof) {
     const size_t T = static_cast<size_t>(prof->n_rows);
-    TRY(dev_upload(e, std::vector<double>(prof->s_max, prof->s_max + ng), &P.s_max));
-    TRY(dev_upload(e, std::vector<double>(prof->pv_std, prof->pv_std + ng), &P.pv_std));
-    TRY(dev_upload(e, std::vector<double>(prof->load_p_std, prof->load_p_std + nl), &P.lp_std));
-    TRY(dev_upload(e, std::vector<double>(prof->load_q_std, prof->load_q_std + nl), &P.lq_std));
+    MAPDN_TRY(dev_upload(e, std::vector<double>(prof->s_max, prof->s_max + ng), &P.s_max));
+    MAPDN_TRY(dev_upload(e, std::vector<double>(prof->pv_std, prof->pv_std + ng), &P.pv_std));
+    MAPDN_TRY(dev_upload(e, std::vector<double>(prof->load_p_std, prof->load_p_std + nl), &P.lp_std));
+    MAPDN_TRY(dev_upload(e, std::vector<double>(prof->load_q_std, prof->load_q_std + nl), &P.lq_std));
     double *dpv, *dlp, *dlq;
-    TRY(dev_alloc(e, T * ng, &dpv)); TRY(dev_alloc(e, T * nl, &dlp)); TRY(dev_alloc(e, T * nl, &dlq));
-    TRY_CUDA(cudaMemcpy(dpv, prof->pv, T * ng * sizeof(double), cudaMemcpyHostToDevice));
+    MAPDN_TRY(dev_alloc(e, T * ng, &dpv)); MAPDN_TRY(dev_alloc(e, T * nl, &dlp)); MAPDN_TRY(dev_alloc(e, T * nl, &dlq));
+    MAPDN_CUDA(cudaMemcpy(dpv, prof->pv, T * ng * sizeof(double), cudaMemcpyHostToDevice));
     if (nl) {
-      TRY_CUDA(cudaMemcpy(dlp, prof->load_p, T * nl * sizeof(double), cudaMemcpyHostToDevice));
-      TRY_CUDA(cudaMemcpy(dlq, prof->load_q, T * nl * sizeof(double), cudaMemcpyHostToDevice));
+      MAPDN_CUDA(cudaMemcpy(dlp, prof->load_p, T * nl * sizeof(double), cudaMemcpyHostToDevice));
+      MAPDN_CUDA(cudaMemcpy(dlq, prof->load_q, T * nl * sizeof(double), cudaMemcpyHostToDevice));
     }
     P.prof_pv = dpv; P.prof_lp = dlp; P.prof_lq = dlq;
     P.n_rows = prof->n_rows; P.steps_per_hour = prof->steps_per_hour;
-    const int episode_days = cfg->episode_limit / (24 * prof->steps_per_hour) + 1;     // reference :397
-    P.n_day_choices = prof->n_days - episode_days;                                     // reference :398
-    if (P.n_day_choices < 1) return bail(fail(MAPDN_ERR_INVALID, "profile store shorter than one episode"));
+    const int episode_days = cfg.episode_limit / (24 * prof->steps_per_hour) + 1;     // reference :397
+    P.n_day_choices = prof->n_days - episode_days;                                    // reference :398
+    if (P.n_day_choices < 1) return fail(MAPDN_ERR_INVALID, "profile store shorter than one episode");
     // the latest sampled window must fit: start_max + episode_limit rows
     const long long last = (static_cast<long long>(P.n_day_choices - 1) * 24 + 23) * prof->steps_per_hour +
-                           (prof->steps_per_hour - 1) + cfg->episode_limit;
-    if (last > prof->n_rows - 1) return bail(fail(MAPDN_ERR_INVALID, "profile store shorter than n_days claims"));
+                           (prof->steps_per_hour - 1) + cfg.episode_limit;
+    if (last > prof->n_rows - 1) return fail(MAPDN_ERR_INVALID, "profile store shorter than n_days claims");
   }
-  P.base_mva = net->base_mva; P.inv_base = 1.0 / net->base_mva;
-  P.vm_init = (net->vm_init > 0) ? net->vm_init : net->slack_vm;
-  P.vm0 = net->slack_vm; P.va0 = net->slack_va_deg * (3.14159265358979323846 / 180.0);
-  P.e0 = P.vm0 * std::cos(P.va0); P.f0 = P.vm0 * std::sin(P.va0);
-  P.ysl_g0 = e->ydiag[2 * slack]; P.ysl_b0 = e->ydiag[2 * slack + 1];
-  P.tol = (cfg->tol > 0) ? cfg->tol : 1e-8;
-  P.max_iter = (cfg->max_iter > 0) ? cfg->max_iter : 10;
-  {
-    // The first Newton iteration starts from the flat start, where S_calc and the Jacobian depend on the network only:
-    // factorise J(V0) once, leaf -> root on the elimination forest, with the formulas of the kernel's edge / mismatch pass
-    // and elimination step (env_kernel.cuh: nr_solve). Per node six double2: S_calc = (P, Q); M = D'^-1 J[i,parent] rows
-    // 0 / 1 (what the back sweep multiplies dx_parent with); D'^-1 rows 0 / 1; J[parent,i] = (a, b).
-    std::vector<double> ft(static_cast<size_t>(12) * std::max(1, npq), 0.0);
-    if (!meshed) {
-      const double* yup = reinterpret_cast<const double*>(hot.data() + hl.yup);
-      const double* ydn = reinterpret_cast<const double*>(hot.data() + hl.ydn);
-      const double* yii = reinterpret_cast<const double*>(hot.data() + hl.yii);
-      // children in a labelling-independent order (first child, second child, then the contiguous extras): the node
-      // relabelling of section 2b must not change a single bit of the results
-      std::vector<std::vector<int>> kids(npq);
-      for (int i = 0; i < npq; ++i) {
-        if (kid0[i] != npq) kids[i].push_back(kid0[i]);
-        if (kid1[i] != npq) kids[i].push_back(kid1[i]);
-        for (int c = 2; c < nchild[i]; ++c) kids[i].push_back(kid1[i] + c - 1);      // extras follow child 1 contiguously
-      }
-      std::vector<int> topo;                               // parents before children
-      for (int i = 0; i < npq; ++i) if (parent[i] < 0) topo.push_back(i);
-      for (size_t qh = 0; qh < topo.size(); ++qh) for (int c : kids[topo[qh]]) topo.push_back(c);
-      const double vi_x = P.vm_init, vi_y = 0.0;             // every PQ bus
-      std::vector<double> upx(npq), upy(npq), dnx(npq), dny(npq), d01x(npq), d01y(npq), d23x(npq), d23y(npq);
-      std::vector<double> s00(npq, 0.0), s01(npq, 0.0), s10(npq, 0.0), s11(npq, 0.0);     // Schur update a bus hands to its parent
-      for (int i = 0; i < npq; ++i) {                      // edge terms of (i, parent); roots: Y = 0
-        const double vp_x = P.vm_init, vp_y = 0.0;
-        const double cc = vi_x * vp_x + vi_y * vp_y, ss = vi_y * vp_x - vi_x * vp_y;
-        upx[i] = yup[2 * i] * ss - yup[2 * i + 1] * cc; upy[i] = yup[2 * i] * cc + yup[2 * i + 1] * ss;
-        dnx[i] = -ydn[2 * i] * ss - ydn[2 * i + 1] * cc; dny[i] = ydn[2 * i] * cc - ydn[2 * i + 1] * ss;
-      }
-      for (int i = 0; i < npq; ++i) {                      // S_calc and the diagonal blocks
-        const double cs0 = vi_x * P.e0 + vi_y * P.f0, sn0 = vi_y * P.e0 - vi_x * P.f0;
-        double sa = ysl_cold[2 * i] * sn0 - ysl_cold[2 * i + 1] * cs0 + upx[i];
-        double sb = ysl_cold[2 * i] * cs0 + ysl_cold[2 * i + 1] * sn0 + upy[i];
-        for (int c : kids[i]) { sa += dnx[c]; sb += dny[c]; }
-        const double vv = vi_x * vi_x + vi_y * vi_y;
-        const double gv = yii[2 * i] * vv, bv = yii[2 * i + 1] * vv;
-        const double Pc = gv + sb, Qc = sa - bv;
-        ft[12 * i + 0] = Pc; ft[12 * i + 1] = Qc;
-        d01x[i] = -Qc - bv; d01y[i] = Pc + gv; d23x[i] = Pc - gv; d23y[i] = Qc - bv;
-      }
-      for (size_t k = topo.size(); k-- > 0;) {              // children before parents
-        const int i = topo[k];
-        for (int c : kids[i]) { d01x[i] -= s00[c]; d01y[i] -= s01[c]; d23x[i] -= s10[c]; d23y[i] -= s11[c]; }
-        const double idet = 1.0 / (d01x[i] * d23y[i] - d01y[i] * d23x[i]);
-        const double ux = upx[i], uy = upy[i], dx = dnx[i], dy = dny[i];
-        const double ma00 = d23y[i] * ux + d01y[i] * uy, ma01 = d23y[i] * uy - d01y[i] * ux;      // adj(D') J[i,parent]
-        const double ma10 = -d23x[i] * ux - d01x[i] * uy, ma11 = d01x[i] * ux - d23x[i] * uy;
-        ft[12 * i + 2] = ma00 * idet; ft[12 * i + 3] = ma01 * idet; ft[12 * i + 4] = ma10 * idet; ft[12 * i + 5] = ma11 * idet;
-        ft[12 * i + 6] = d23y[i] * idet; ft[12 * i + 7] = -d01y[i] * idet;                         // D'^-1
-        ft[12 * i + 8] = -d23x[i] * idet; ft[12 * i + 9] = d01x[i] * idet;
-        ft[12 * i + 10] = dx; ft[12 * i + 11] = dy;
-        s00[i] = (dx * ma00 + dy * ma10) * idet; s01[i] = (dx * ma01 + dy * ma11) * idet;         // J[parent,i] D'^-1 J[i,parent]
-        s10[i] = (dx * ma10 - dy * ma00) * idet; s11[i] = (dx * ma11 - dy * ma01) * idet;
-      }
-    }
-    const double* d_ft = nullptr;
-    TRY(dev_upload(e, ft, &d_ft));
-    P.first_tab = reinterpret_cast<const double2*>(d_ft);
-  }
-  P.barrier = cfg->barrier; P.voltage_weight = cfg->voltage_weight; P.q_weight = cfg->q_weight;
-  P.line_weight = cfg->line_weight; P.use_line_weight = cfg->use_line_weight;
-  P.v_upper = cfg->v_upper; P.v_lower = cfg->v_lower; P.episode_limit = cfg->episode_limit;
-  P.action_low = cfg->action_low; P.action_high = cfg->action_high; P.reset_action = cfg->reset_action;
-  P.seed = cfg->seed; P.env_id_offset = cfg->env_id_offset;
-  TRY(dev_alloc(e, B * nl, &P.cur_pl)); TRY(dev_alloc(e, B * nl, &P.cur_ql));
-  TRY(dev_alloc(e, B * ng, &P.cur_pv)); TRY(dev_alloc(e, B * ng, &P.cur_q));
-  TRY(dev_alloc(e, B * n, &P.res_vm)); TRY(dev_alloc(e, B * n, &P.res_va));
-  TRY(dev_alloc(e, B * n, &P.res_p)); TRY(dev_alloc(e, B * n, &P.res_q));
-  TRY(dev_alloc(e, B * std::max(1, n_line), &P.res_pl));
-  TRY(dev_alloc(e, B, &P.steps)); TRY(dev_alloc(e, B, &P.sum_rewards));
-  TRY(dev_alloc(e, B, &P.start_row)); TRY(dev_alloc(e, B, &P.episode)); TRY(dev_alloc(e, B, &P.nr_iters));
-  if (meshed) {
+  P.base_mva = net.base_mva; P.inv_base = 1.0 / net.base_mva;
+  P.vm_init = v0.vm_init; P.vm0 = v0.vm0; P.va0 = v0.va0; P.e0 = v0.e0; P.f0 = v0.f0;
+  P.ysl_g0 = y.ydiag[2 * slack]; P.ysl_b0 = y.ydiag[2 * slack + 1];
+  P.tol = (cfg.tol > 0) ? cfg.tol : 1e-8;
+  P.max_iter = (cfg.max_iter > 0) ? cfg.max_iter : 10;
+  P.barrier = cfg.barrier; P.voltage_weight = cfg.voltage_weight; P.q_weight = cfg.q_weight;
+  P.line_weight = cfg.line_weight; P.use_line_weight = cfg.use_line_weight;
+  P.v_upper = cfg.v_upper; P.v_lower = cfg.v_lower; P.episode_limit = cfg.episode_limit;
+  P.action_low = cfg.action_low; P.action_high = cfg.action_high; P.reset_action = cfg.reset_action;
+  P.seed = cfg.seed; P.env_id_offset = cfg.env_id_offset;
+  MAPDN_TRY(dev_alloc(e, B * nl, &P.cur_pl)); MAPDN_TRY(dev_alloc(e, B * nl, &P.cur_ql));
+  MAPDN_TRY(dev_alloc(e, B * ng, &P.cur_pv)); MAPDN_TRY(dev_alloc(e, B * ng, &P.cur_q));
+  MAPDN_TRY(dev_alloc(e, B * n, &P.res_vm)); MAPDN_TRY(dev_alloc(e, B * n, &P.res_va));
+  MAPDN_TRY(dev_alloc(e, B * n, &P.res_p)); MAPDN_TRY(dev_alloc(e, B * n, &P.res_q));
+  MAPDN_TRY(dev_alloc(e, B * std::max(1, t.n_line), &P.res_pl));
+  MAPDN_TRY(dev_alloc(e, B, &P.steps)); MAPDN_TRY(dev_alloc(e, B, &P.sum_rewards));
+  MAPDN_TRY(dev_alloc(e, B, &P.start_row)); MAPDN_TRY(dev_alloc(e, B, &P.episode)); MAPDN_TRY(dev_alloc(e, B, &P.nr_iters));
+  if (f.meshed) {
     const size_t m = 2 * static_cast<size_t>(npq);
     P.dense_stride = static_cast<int>(m * (m + 1));
-    const size_t groups = static_cast<size_t>(e->max_blocks) * e->epb;       // one slice per resident env group
-    TRY(dev_alloc(e, groups * P.dense_stride, &P.dense_ws));
+    const size_t groups = static_cast<size_t>(e->max_blocks_step[0][0]) * e->epb;       // one slice per resident env group
+    MAPDN_TRY(dev_alloc(e, groups * P.dense_stride, &P.dense_ws));
   }
   // staging for the *_host entry points
-  TRY(dev_alloc(e, B * ng, &e->d_stage_actions)); TRY(dev_alloc(e, B, &e->d_stage_reward)); TRY(dev_alloc(e, B, &e->d_stage_term));
-  TRY(dev_alloc(e, B * MAPDN_N_INFO, &e->d_stage_info)); TRY(dev_alloc(e, B * std::max<size_t>(ng * obs_dim, e->compact_row), &e->d_stage_obs));   // compact rows round up to 4 entries
+  MAPDN_TRY(dev_alloc(e, B * ng, &e->d_stage_actions)); MAPDN_TRY(dev_alloc(e, B, &e->d_stage_reward)); MAPDN_TRY(dev_alloc(e, B, &e->d_stage_term));
+  MAPDN_TRY(dev_alloc(e, B * MAPDN_N_INFO, &e->d_stage_info));
+  MAPDN_TRY(dev_alloc(e, B * std::max<size_t>(ng * o.obs_dim, e->compact_row), &e->d_stage_obs));   // compact rows round up to 4 entries
 
   mapdn_dims& d = e->dims;
-  d.batch = cfg->batch; d.n_bus = n; d.n_branch = nbr; d.n_line = n_line; d.n_load = nl; d.n_sgen = ng;
-  d.n_agents = ng; d.n_actions = 1; d.obs_dim = obs_dim; d.state_dim = P.state_dim; d.n_info = MAPDN_N_INFO;
-  d.lanes_per_env = G; d.envs_per_block = e->epb; d.smem_bytes = e->smem; d.n_levels = n_lev;
+  d.batch = cfg.batch; d.n_bus = n; d.n_branch = net.n_branch; d.n_line = t.n_line; d.n_load = nl; d.n_sgen = ng;
+  d.n_agents = ng; d.n_actions = 1; d.obs_dim = o.obs_dim; d.state_dim = P.state_dim; d.n_info = MAPDN_N_INFO;
+  d.lanes_per_env = e->G; d.envs_per_block = e->epb; d.smem_bytes = e->smem; d.n_levels = f.n_lev;
   // SURVEY §8d: read p_load,q_load,p_pv,a ; write vm,va ; write obs ; reward+done+11 info
-  d.algorithmic_bytes_per_env_step = 8LL * (2 * nl + 2 * ng) + 8LL * 2 * n + 8LL * ng * obs_dim + 8LL * 13;
+  d.algorithmic_bytes_per_env_step = 8LL * (2 * nl + 2 * ng) + 8LL * 2 * n + 8LL * ng * o.obs_dim + 8LL * 13;
+  return MAPDN_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int32_t mapdn_abi_version(void) { return MAPDN_ABI_VERSION; }
+const char* mapdn_last_error(void) { return g_last_error.c_str(); }
+
+mapdn_status mapdn_destroy(mapdn_env* e) {
+  if (!e) return MAPDN_OK;
+  DeviceGuard guard(e->device);
+  for (void* d : e->allocs) cudaFree(d);
+  delete e;
+  return MAPDN_OK;
+}
+
+mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* prof, const mapdn_cfg* cfg,
+                          int32_t device, mapdn_env** out) {
+  if (!net || !cfg || !out) return fail(MAPDN_ERR_INVALID, "null argument");
+  *out = nullptr;
+  MAPDN_TRY(validate_create_args(net, prof, cfg));
+  MAPDN_ON_DEVICE(device);
+  // owns the half-built handle: every refusal below frees it and its device memory
+  std::unique_ptr<mapdn_env, decltype(&mapdn_destroy)> e(new (std::nothrow) mapdn_env(), &mapdn_destroy);
+  if (!e) return fail(MAPDN_ERR_NOMEM, "out of host memory");
+  e->device = device;
+  e->cfg = *cfg;
+  const int n = net->n_bus, nl = net->n_load, ng = net->n_sgen;
+
+  Ybus y;
+  MAPDN_TRY(ybus_on_device(e.get(), *net, y));
+  Forest f;
+  MAPDN_TRY(build_forest(y, n, net->slack_bus, f));
+  Sweeps s;
+  MAPDN_TRY(plan_sweeps(f, cfg->lanes_per_env, s));
+  relabel_nodes(y, f, s);
+  const ElementMaps m = element_maps(*net, f);
+  ObsPrograms o;
+  MAPDN_TRY(obs_programs(*net, f, s.G, cfg->state_space_mask, o));
+  const BranchTables t = branch_tables(y, f, net->base_mva);
+  const HotBlob hot = build_hot_blob(y, f, s, m, o, t);
+  cudaDeviceProp dp{};
+  MAPDN_CUDA(cudaGetDeviceProperties(&dp, device));
+  Geometry geo;
+  MAPDN_TRY(plan_geometry(n - 1, ng, nl, s.G, cfg->batch, hot.bytes_core, hot.bytes_full, dp.sharedMemPerBlockOptin,
+                          dp.multiProcessorCount, geo));
+  const FlatStart v0 = flat_start(*net);
+  const std::vector<double> ft = first_iteration_factors(f, hot, v0);
+
+  e->dense = f.meshed;
+  e->G = s.G; e->threads = geo.epb * s.G; e->epb = geo.epb; e->smem = geo.smem; e->helper_threads = geo.helper_threads;
+  MAPDN_TRY(size_kernels(e.get(), dp));
+  MAPDN_TRY(upload_plan(e.get(), *net, prof, y, f, s, o, t, hot, geo, v0, ft));
   // the memsets / uploads above ran on the legacy default stream: order them before any launch of the caller's
   // (possibly non-blocking) streams
-  TRY_CUDA(cudaDeviceSynchronize());
-  *out = e;
+  MAPDN_CUDA(cudaDeviceSynchronize());
+  *out = e.release();
   return MAPDN_OK;
-#undef TRY
-#undef TRY_CUDA
 }
 
 mapdn_status mapdn_get_dims(const mapdn_env* e, mapdn_dims* out) {

@@ -8,7 +8,7 @@ compared with the oracle (tests/geometry_cases.py; the oracle runs over a proces
 The matrix on the device: forced plans 0-3, helper warps 1 and 4, small and default envs per CTA for case141 x 2048 and
 case322 x 1024, each needing at least two rounds, must give bit-identical outputs (and so match the oracle too).
 
-The record instantiation's own persistent grid (max_blocks_record) never needs more rounds than the plain step's at the
+The record instantiation's own persistent grid (max_blocks_step[0][1]) never needs more rounds than the plain step's at the
 planner's geometries: for G <= 32 it holds 165-166 registers instead of 130-134 (168 vs 136 allocated, 5376 vs 4352 per
 warp), so a CTA of W warps fits floor(12.19 / W) times instead of floor(15.06 / W) by registers - fewer only for W = 2, 3,
 5 or 7. The planner picks a CTA size that finishes the batch in one round of <= 132 CTAs whenever that fits (1 CTA per SM
