@@ -277,6 +277,27 @@ mapdn_status mapdn_step_stacked(mapdn_env* env, const double* actions_dev /*[B,n
                                 double* record_dev /*or NULL*/, int64_t record_stride, void* stream);
 mapdn_status mapdn_get_obs_stacked(mapdn_env* env, double* obs_stacked_dev, void* stream);
 
+/*
+ * Step with auto-reset: an env that terminates in the step (steps >= episode_limit or a diverged power flow) starts its
+ * next episode in the same launch. One launch whose results equal, call for call, those of
+ *   1. mapdn_step (obs_stacked_dev NULL) / mapdn_step_stacked with the same arguments (no records);
+ *   2. mapdn_reset(env, NULL, mask = terminated_dev, add_noise = 1, obs = reset_obs_dev, state = NULL,
+ *      converged = reset_ok_dev): sampled start, noise on, up to the reset's own number of draws; an env whose draws
+ *      all diverge keeps its power-flow results (res_*) and, like any reset env, starts the new episode's counters
+ *      (steps = 1, sum_rewards, start_row, episode) with the element values of its last draw;
+ *   3. with history, mapdn_get_obs_stacked into reset_obs_stacked_dev, for the terminated envs.
+ * obs_dev / obs_stacked_dev keep the step's (terminal) observation; reset_obs_dev [B,n_agents,obs_dim],
+ * reset_obs_stacked_dev [B,n_agents,H*obs_dim] and reset_ok_dev [B] are written for the terminated envs only (each may
+ * be NULL). Refuses a null handle, actions, reward or terminated, a handle without a profile store, and stacked
+ * pointers on a handle without history.
+ */
+mapdn_status mapdn_step_autoreset(mapdn_env* env, const double* actions_dev /*[B,n_sgen]*/, int32_t add_noise,
+                                  double* reward_dev /*[B]*/, uint8_t* terminated_dev /*[B]*/,
+                                  double* info_dev /*[B,11] or NULL*/, double* obs_dev /*or NULL*/,
+                                  double* obs_stacked_dev /*or NULL*/, double* reset_obs_dev /*or NULL*/,
+                                  double* reset_obs_stacked_dev /*or NULL*/, uint8_t* reset_ok_dev /*or NULL*/,
+                                  void* stream);
+
 mapdn_status mapdn_get_obs(mapdn_env* env, double* obs_dev, void* stream);      /* :232-316 */
 mapdn_status mapdn_get_state(mapdn_env* env, double* state_dev, void* stream);  /* :213-230 */
 mapdn_status mapdn_get_field(mapdn_env* env, int32_t field, double* out_dev, void* stream);

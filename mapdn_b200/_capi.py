@@ -81,6 +81,7 @@ SIGNATURES = dict(
     mapdn_obs_compact_layout=([_vp] * 4, _i32), mapdn_record_layout=([_vp] * 3, _i32),
     mapdn_record=([_vp, _vp, _i64, _vp], _i32), mapdn_set_history=([_vp, _i32], _i32),
     mapdn_step_stacked=(_STEP[:-1] + [_vp, _vp, _i64, _vp], _i32), mapdn_get_obs_stacked=([_vp] * 3, _i32),
+    mapdn_step_autoreset=(_STEP[:-1] + [_vp] * 5, _i32),
     mapdn_get_obs=([_vp] * 3, _i32), mapdn_get_state=([_vp] * 3, _i32),
     mapdn_get_field=([_vp, _i32, _vp, _vp], _i32), mapdn_solve=([_vp, _i32] + [_vp] * 12, _i32),
     mapdn_droop=([_vp, _i32] + [_vp] * 5 + [C.c_double, C.c_double, _i32] + [_vp] * 5, _i32),

@@ -790,15 +790,38 @@ __device__ __forceinline__ void write_stacked_row(const Params& p, int env, int 
   }
 }
 
+// entry idx of get_obs() of env `env` from the state in HBM (reference :232-316), driven by the precomputed obs program
+__device__ __forceinline__ double obs_entry(const Params& p, int env, int idx) {
+  const size_t eN = static_cast<size_t>(env) * p.n_bus, eG = static_cast<size_t>(env) * p.n_sgen;
+  const unsigned src = __ldg(p.obs_src + idx);   // cold copy of the obs program (kind | node)
+  const int kind = static_cast<int>(src >> 28), ix = static_cast<int>(src & 0x0FFFFFFFu);
+  // node id -> bus id (npq = slack)
+  auto bus = [&](int i) { return (i == p.npq) ? p.slack_bus : __ldg(p.bus_of_node + i); };
+  double v = 0.0;
+  if (kind == OBS_P || kind == OBS_Q) {
+    v = (kind == OBS_P) ? p.res_p[eN + bus(ix)] : p.res_q[eN + bus(ix)];
+    for (int t = __ldg(p.obs_xptr + idx), te = __ldg(p.obs_xptr + idx + 1); t < te; ++t) {
+      const int sg = __ldg(p.obs_xidx + t);
+      v += (kind == OBS_P) ? p.cur_pv[eG + sg] : p.cur_q[eG + sg];
+    }
+  } else if (kind == OBS_PV) v = p.cur_pv[eG + ix];
+  else if (kind == OBS_QSG) v = p.cur_q[eG + ix];
+  else if (kind == OBS_VM) v = p.res_vm[eN + bus(ix)];
+  else if (kind == OBS_VA) v = p.res_va[eN + bus(ix)];
+  return v;
+}
+
 // RECORD (MODE_STEP only): the epilogue also writes the env's tester record row (see Params::record) from the values it
 // already holds. HIST (MODE_STEP only, handles with history): the epilogue also writes the env's newest observation frame
-// into its slot of the ring and, when Params::obs_stacked is set, the stacked row. Template flags, so the instantiations
-// without them are the same code as before they existed.
-template <int G, int MODE, bool DENSE = false, bool RECORD = false, bool HIST = false>
+// into its slot of the ring and, when Params::obs_stacked is set, the stacked row. AUTORESET (MODE_STEP only, not with
+// RECORD): after the step, every env that terminated runs the reset of MODE_RESET in the same launch (see the end of the
+// persistent loop). Template flags, so the instantiations without them are the same code as before they existed.
+template <int G, int MODE, bool DENSE = false, bool RECORD = false, bool HIST = false, bool AUTORESET = false>
 __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_constant__ Params p) {
   static_assert(!DENSE || G == 32, "the dense fallback uses one warp per env");
   static_assert(!RECORD || MODE == MODE_STEP, "records are written by the step kernel");
   static_assert(!HIST || MODE == MODE_STEP, "the frame ring is written by the step kernel (resets: reset_frame_kernel)");
+  static_assert(!AUTORESET || (MODE == MODE_STEP && !RECORD), "auto-reset follows a step without tester records");
   static_assert(G == 4 || G == 8 || G == 16 || G == 32 || G == 64 || G == 128, "unsupported group size");
 #ifdef MAPDN_HOST_EMU
   unsigned char* const smem_raw = emu::dyn_smem();
@@ -878,7 +901,14 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
   double* stage_lin = s.scratch + ng + (G > 32 ? 10 * (G / 32) : 0);
   const uint32_t k0 = static_cast<uint32_t>(p.seed), k1 = static_cast<uint32_t>(p.seed >> 32);
 
-  for (int base = blockIdx.x * epb; base < p.nb; base += gridDim.x * epb) {
+  // AUTORESET: after the step pass over the envs of a round, a warp (G <= 32) or group (G > 32) with an env that terminated
+  // runs a reset pass over the same envs (see below) before it moves to the next round
+  bool ended = false;         // MODE_STEP: the group's env terminated in the step pass
+  bool reset_next = false;    // the next iteration is the reset pass over the envs of this round
+  // (AUTORESET spelled out in the two expressions below: the other instantiations keep the loop exactly as it was)
+  for (int base = blockIdx.x * epb; base < p.nb; base += (AUTORESET && reset_next) ? 0 : gridDim.x * epb) {
+    const bool auto_pass = AUTORESET && reset_next;
+    reset_next = false;
     if (is_helper) {
       // ---- helper warps: next profile row of every env of this round (reference _set_demand_and_pv :491-513:
       //      t = self.steps before the increment) + |N(0,1)| * std noise in Box-Muller pairs (2m, 2m+1) over the
@@ -969,10 +999,18 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
       named_bar_arrive(2, blockDim.x);                 // new pv of every env is in shared memory
       continue;
     }
+    // The pass runs in mode M: the kernel's own MODE, or MODE_RESET in the auto-reset pass, so that a launched reset and an
+    // auto-reset run the same code. The auto-reset pass differs from a reset launch only where the step launch's
+    // parameters say otherwise: the selection is `ended`, the start is sampled and noise is on (reference reset() :118),
+    // the observation goes to Params::reset_obs, and frame 0 of the new episode to the ring and Params::reset_obs_stacked.
+    // (One loop body for both passes, not a function instantiated per mode: the instantiations without AUTORESET keep their
+    // code as it was.)
+    const int M = auto_pass ? static_cast<int>(MODE_RESET) : MODE;
     int env = base + gidx;
     bool valid = env < p.nb;
     if (!valid) env = p.nb - 1;
-    if (MODE == MODE_RESET && p.mask != nullptr && !p.mask[env]) valid = false;
+    if (auto_pass) { if (!ended) valid = false; }
+    else if (M == MODE_RESET && p.mask != nullptr && !p.mask[env]) valid = false;
     const size_t eL = static_cast<size_t>(env) * nl, eG = static_cast<size_t>(env) * ng,
                  eN = static_cast<size_t>(env) * n;
 
@@ -981,12 +1019,12 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
     int steps_old = 0;
     // (groups beyond the batch work on a clamped env id without storing anything: they must not read the scalars that the
     // env's real group rewrites at the end of its step / reset - a benign race, but a race)
-    if (MODE == MODE_STEP && valid) {
+    if (M == MODE_STEP && valid) {
       key.c3base = p.episode[env] * 8u;
       start = p.start_row[env];
       steps_old = p.steps[env];
     }
-    if (MODE == MODE_RESET && valid) key.c3base = (p.episode[env] + 1u) * 8u;
+    if (M == MODE_RESET && valid) key.c3base = (p.episode[env] + 1u) * 8u;
 
     bool conv = false;
     int iters = 0;
@@ -995,12 +1033,12 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
     bool dr_active = valid;      // MODE_DROOP: this env has not met the stopping rule yet
     int dr_iters = 0;
     double* v_last = s.scratch;                    // MODE_DROOP: PV-bus voltages of the previous power flow [n_sgen]
-    const int n_rounds = (MODE == MODE_RESET) ? kMaxResetAttempts : (MODE == MODE_DROOP ? p.droop_max_ite : 1);
+    const int n_rounds = (M == MODE_RESET) ? kMaxResetAttempts : (M == MODE_DROOP ? p.droop_max_ite : 1);
     for (int round = 0; round < n_rounds; ++round) {
       // ---------------- prologue: element values -> sgen p/q and bus injections ----------------
-      if (MODE == MODE_RESET) {
+      if (M == MODE_RESET) {
         int day, hour, interval;
-        if (p.start_dhi != nullptr) {                               // manual_reset :137-152
+        if (!auto_pass && p.start_dhi != nullptr) {                 // manual_reset :137-152
           day = p.start_dhi[env * 3 + 0]; hour = p.start_dhi[env * 3 + 1]; interval = p.start_dhi[env * 3 + 2];
         } else {                                                    // :111-113, :381-398
           const u32x4 r = philox4x32_10(0u, static_cast<uint32_t>(attempt), key.env, key.c3base + kStreamTime, k0, k1);
@@ -1015,22 +1053,22 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
         start = max(0ll, min(start, p.n_rows - 1 - p.episode_limit));
       }
       long long row = 0;
-      if (MODE == MODE_RESET) { row = start + 1; if (row > p.n_rows - 1) row = p.n_rows - 1; }   // t = steps = 1
+      if (M == MODE_RESET) { row = start + 1; if (row > p.n_rows - 1) row = p.n_rows - 1; }   // t = steps = 1
       const uint32_t c1 = kResetFlag | static_cast<uint32_t>(attempt);
       // (1) coalesced, independent loads of the env's element values into shared memory
-      if (MODE != MODE_DROOP || round == 0) {          // droop: later rounds only change q (in shared memory)
+      if (M != MODE_DROOP || round == 0) {          // droop: later rounds only change q (in shared memory)
 #pragma unroll 4
       for (int j = gl; j < ng; j += G) {
         double pv, q;
-        if (MODE == MODE_SOLVE || MODE == MODE_DROOP) {
-          pv = p.in_pv[eG + j]; q = (MODE == MODE_SOLVE) ? p.in_q[eG + j] : 0.0;     // droop starts from q = 0 (:107)
-          if (MODE == MODE_DROOP) v_last[j] = 100.0;                                    // :123
-        } else if (MODE == MODE_STEP) {
+        if (M == MODE_SOLVE || M == MODE_DROOP) {
+          pv = p.in_pv[eG + j]; q = (M == MODE_SOLVE) ? p.in_q[eG + j] : 0.0;     // droop starts from q = 0 (:107)
+          if (M == MODE_DROOP) v_last[j] = 100.0;                                    // :123
+        } else if (M == MODE_STEP) {
           pv = p.cur_pv[eG + j];
           q = clip_q(p.actions[eG + j], pv, __ldg(p.s_max + j));             // :553
         } else {
           pv = __ldg(p.prof_pv + row * ng + j);
-          if (p.add_noise) pv += __ldg(p.pv_std + j) * half_normal(key, c1, j);   // :498
+          if (auto_pass || p.add_noise) pv += __ldg(p.pv_std + j) * half_normal(key, c1, j);   // :498
           q = 0.0;
           if (p.reset_action) {                                               // :120-122, :334-338
             const u32x4 r = philox4x32_10(j, static_cast<uint32_t>(attempt), key.env, key.c3base + kStreamAction, k0, k1);
@@ -1049,12 +1087,12 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
 #pragma unroll 4
         for (int l = gl; l < nl; l += G) {
           double pl, ql;
-          if (MODE == MODE_SOLVE || MODE == MODE_DROOP) { pl = p.in_pl[eL + l]; ql = p.in_ql[eL + l]; }
-          else if (MODE == MODE_STEP) { pl = p.cur_pl[eL + l]; ql = p.cur_ql[eL + l]; }
+          if (M == MODE_SOLVE || M == MODE_DROOP) { pl = p.in_pl[eL + l]; ql = p.in_ql[eL + l]; }
+          else if (M == MODE_STEP) { pl = p.cur_pl[eL + l]; ql = p.cur_ql[eL + l]; }
           else {
             pl = __ldg(p.prof_lp + row * nl + l);
             ql = __ldg(p.prof_lq + row * nl + l);
-            if (p.add_noise) {                                                   // :503, :508
+            if (auto_pass || p.add_noise) {                                      // :503, :508
               pl += __ldg(p.lp_std + l) * half_normal(key, c1, ng + l);
               ql += __ldg(p.lq_std + l) * half_normal(key, c1, ng + nl + l);
             }
@@ -1082,7 +1120,7 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
       if (stage_rec) stage_and_gather([&](int k) -> double* { return s.base + (k / 12) * (2 * kNodeArrays2) + 2 * A_UP + (k % 12); });
       else stage_and_gather([&](int k) -> double* { return stage_lin + k; });
       grp_sync<G>(gidx);
-      if (MODE == MODE_STEP) named_bar_arrive(1, blockDim.x);   // the current rows are consumed: the helper may overwrite them
+      if (M == MODE_STEP) named_bar_arrive(1, blockDim.x);   // the current rows are consumed: the helper may overwrite them
 
       // ---------------- Newton-Raphson ----------------
       PROF(1)
@@ -1097,7 +1135,7 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
 #endif
       }
       PROF(4)
-      if (MODE == MODE_DROOP) {
+      if (M == MODE_DROOP) {
         // relaxed fixed-point loop of pf_droop_matpower_all.m:121-152: stop when ||v_pv - v_pv_last||_2 < tol, else
         // q <- (1 - gain) q + gain q_droop(v). An env that has stopped keeps its q, so the power flows it still runs
         // alongside the others of its warp reproduce its final state; the last allowed round does not move q either
@@ -1123,7 +1161,7 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
         grp_sync<G>(gidx);
         continue;
       }
-      if (MODE != MODE_RESET) break;
+      if (M != MODE_RESET) break;
       if (conv) solved = true;
       if (grp_exit<G>(solved)) break;
       if (!solved) ++attempt;                       // re-draw this env (reference retry loop :108-133)
@@ -1132,7 +1170,7 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
 
     // ---------------- epilogue ----------------
     // divergence branch (reference :188-196): fall back to the previous solution kept in HBM
-    if (MODE == MODE_STEP && !conv) {
+    if (M == MODE_STEP && !conv) {
       for (int i = gl; i < npq; i += G) {
         const int b = __ldg(p.bus_of_node + i);
         const double vm = p.res_vm[eN + b], va = p.res_va[eN + b];
@@ -1146,9 +1184,9 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
     }
     grp_sync<G>(gidx);
     // a reset whose kMaxResetAttempts draws all diverged keeps the env's previous state and reports it (reset_ok)
-    constexpr bool kExplicit = (MODE == MODE_SOLVE || MODE == MODE_DROOP);     // explicit inputs / outputs, no env state
+    const bool kExplicit = (M == MODE_SOLVE || M == MODE_DROOP);     // explicit inputs / outputs, no env state
     const bool write_res = valid && (kExplicit || conv);
-    if (MODE == MODE_RESET && valid && gl == 0 && p.reset_ok != nullptr) p.reset_ok[env] = conv ? 1 : 0;
+    if (M == MODE_RESET && valid && gl == 0 && p.reset_ok != nullptr) p.reset_ok[env] = conv ? 1 : 0;
     if (!kExplicit && valid && gl == 0) p.nr_iters[env] = conv ? iters : p.max_iter;
 
     // slack injection (pfsoln, SURVEY A.5): S0 = V0 conj(Ybus[0,:] V) -> sentinel record's SP
@@ -1168,7 +1206,7 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
     PROF(7)
     // sgen.q_mvar after the step: the clipped action, or the previous q on divergence (:189-196)
     double sum_q_eff = 0.0, sum_q_try = 0.0;
-    if (MODE == MODE_STEP) {
+    if (M == MODE_STEP) {
       for (int j = gl; j < ng; j += G) {
         const double q_try = s.q[j];
         const double q_eff = conv ? q_try : p.cur_q[eG + j];
@@ -1183,8 +1221,8 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
     // record row [pv | q | P_bus | Q_bus | vm | line loss] (the order of the reference tester's getters): exactly what
     // mapdn_get_field returns after this step. pv is already the next profile row (reference :199 runs before the
     // tester's getters); q is the effective one; a diverged env reports its previous results, read back from HBM.
-    double* const rec = RECORD ? p.record + static_cast<size_t>(env) * p.record_stride : nullptr;
-    if (MODE == MODE_STEP) {
+    [[maybe_unused]] double* const rec = RECORD ? p.record + static_cast<size_t>(env) * p.record_stride : nullptr;
+    if (M == MODE_STEP) {
       named_bar_sync(2, blockDim.x);
       for (int j = gl; j < ng; j += G) s.pv[j] = next_row[j];
       if constexpr (RECORD) {
@@ -1236,7 +1274,7 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
             rec[2 * ng + 2 * n + b] = v;                    // on divergence: reloaded from res_vm above
           }
         }
-        if (MODE == MODE_STEP) {
+        if (M == MODE_STEP) {
           cnt_lo += (v < p.v_lower) ? 1.0 : 0.0;
           cnt_hi += (v > p.v_upper) ? 1.0 : 0.0;
           sum_dev += fabs(v - v_ref);
@@ -1273,7 +1311,7 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
     }
     PROF(9)
     if (kExplicit) {
-      if (MODE == MODE_DROOP) {
+      if (M == MODE_DROOP) {
         double tot[1] = {sum_pl};
         const bool no_max[1] = {false};
         grp_reduce<G, 1>(gidx, gl, tot, no_max, red_scratch);
@@ -1283,14 +1321,14 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
         }
       }
       if (valid && gl == 0) {
-        if (MODE == MODE_SOLVE && p.out_iters) p.out_iters[env] = conv ? iters : p.max_iter;
+        if (M == MODE_SOLVE && p.out_iters) p.out_iters[env] = conv ? iters : p.max_iter;
         if (p.out_conv) p.out_conv[env] = conv ? 1 : 0;
       }
       grp_sync<G>(gidx);
       continue;
     }
 
-    if (MODE == MODE_STEP) {
+    if (M == MODE_STEP) {
       {
         double rv[10] = {cnt_lo, cnt_hi, sum_dev, sum_v, sum_bar, max_drop, max_rise, sum_pl, sum_q_eff, sum_q_try};
         const bool rmax[10] = {false, false, false, false, false, true, true, false, false, false};
@@ -1313,6 +1351,7 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
         p.steps[env] = steps_new;
         p.sum_rewards[env] += reward;                                           // :203
       }
+      ended = valid && (steps_new >= p.episode_limit || !conv);
       if (valid && p.info != nullptr) {
         // the 11 info scalars, one per lane (every lane of the group holds the reduced values): one or two store
         // instructions per env instead of eleven from lane 0 - it matters when `info` is pinned host memory
@@ -1342,16 +1381,17 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
     // instruction (two fp64 / four fp32 entries) and consecutive lanes consecutive 16-byte pieces, so one store
     // instruction writes 128 contiguous bytes per env (full lines when the destination is pinned host memory).
     // obs_skip_off: entries reading that slot (the padding) are not stored.
-    if ((p.obs != nullptr || (MODE == MODE_STEP && p.obs32 != nullptr)) && valid) {
+    // (the destination is spelled out at each use: a local copy of p.obs would change the code of the other instantiations)
+    if (((auto_pass ? p.reset_obs : p.obs) != nullptr || (M == MODE_STEP && p.obs32 != nullptr)) && valid) {
       const bool compact = p.obs_compact_len > 0;          // rows without the per-agent padding (staged host path)
       const int tot = compact ? p.obs_compact_len : ng * p.obs_dim;
       const int skip = p.obs_skip_off;
       auto gather = [&](const uint16_t* __restrict__ prog, auto cold) {   // prog: shared (blob) or global (cold copy: read-only path)
         constexpr bool kCold = decltype(cold)::value;
         int done_to = 0;
-        if (p.obs != nullptr) {
-          double* o = p.obs + static_cast<size_t>(env) * tot;
-          if ((tot & 1) == 0 && (reinterpret_cast<uintptr_t>(p.obs) & 15) == 0) {
+        if ((auto_pass ? p.reset_obs : p.obs) != nullptr) {
+          double* o = (auto_pass ? p.reset_obs : p.obs) + static_cast<size_t>(env) * tot;
+          if ((tot & 1) == 0 && (reinterpret_cast<uintptr_t>(auto_pass ? p.reset_obs : p.obs) & 15) == 0) {
             const uint32_t* offv = reinterpret_cast<const uint32_t*>(prog);
             const int npair = tot >> 1;
 #pragma unroll (kCold ? 8 : 4)
@@ -1397,7 +1437,27 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
       if (h.in_blob && !compact) gather(reinterpret_cast<const uint16_t*>(smem_raw + hl.obs_off), std::false_type{});
       else gather(compact ? p.obs_compact_prog : p.obs_off, std::true_type{});
     }
-    if constexpr (HIST) {
+    if (HIST && AUTORESET && auto_pass) {
+      // frame 0 of the new episode, what reset_frame_kernel writes after a reset launch: the slab through the padded
+      // program when the reset converged (the state in HBM holds the same values), else the state in HBM (a reset whose
+      // draws all diverged keeps the old res_*, which its slab does not hold; the group's stores above must be visible to
+      // every lane of the group first). Its stacked row (write_stacked_row at f = 0): H - 1 zero frames, then frame 0.
+      grp_sync<G>(gidx);
+      if (valid) {
+        const int od = p.obs_dim, tot = ng * od, blk = p.history * od;
+        const uint16_t* prog = h.in_blob ? reinterpret_cast<const uint16_t*>(smem_raw + hl.obs_off) : p.obs_off;
+        auto frame0 = [&](int i) { return conv ? s.base[prog[i]] : obs_entry(p, env, i); };
+        double* fr = p.hist + static_cast<size_t>(env) * p.history * tot;
+        for (int i = gl; i < tot; i += G) fr[i] = frame0(i);
+        if (p.reset_obs_stacked != nullptr) {
+          double* o = p.reset_obs_stacked + static_cast<size_t>(env) * ng * blk;
+          for (int e = gl; e < ng * blk; e += G) {
+            const int a = e / blk, r = e - a * blk;
+            o[e] = r < blk - od ? 0.0 : frame0(a * od + r - (blk - od));
+          }
+        }
+      }
+    } else if constexpr (HIST) {
       // frame f = steps - 1 of this step into its ring slot, through the padded program whatever layout (compact, fp32,
       // none) the caller's observations take; then the stacked row, whose newest frame comes straight from the slab
       if (valid) {
@@ -1413,7 +1473,7 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
         if (p.obs_stacked != nullptr) write_stacked_row(p, env, f, gl, G, [&](int i) { return s.base[prog[i]]; });
       }
     }
-    if (MODE == MODE_RESET && p.state != nullptr) {
+    if (M == MODE_RESET && !auto_pass && p.state != nullptr) {
       // get_state (:213-230): [P_bus | Q_bus | pv | q | vm | va(deg)] restricted to state_space (cold program)
       double* o = p.state + static_cast<size_t>(env) * p.state_dim;
       for (int idx = gl; idx < p.state_dim; idx += G) {
@@ -1431,6 +1491,16 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
     }
     grp_sync<G>(gidx);
     PROF(11)
+    if constexpr (AUTORESET) if (!auto_pass) {
+      // The reset pass adds no arrivals at the named barriers 1 and 2: the helper warps draw the step's next rows only, and
+      // their stores to cur_* of this round's envs are ordered before the step pass's wait at barrier 2 (bar.arrive after
+      // __threadfence_block), so the reset pass overwrites them. Its entry must be uniform where the group primitives are
+      // wider than the group: for G <= 32 they use full-warp masks, so the whole warp enters when one of its groups
+      // terminated (the others take part with valid = false, like envs outside the mask of a reset launch); for G > 32
+      // `ended` is already uniform over the group (named barrier 3 + gidx).
+      reset_next = ended;
+      if constexpr (G <= 32) reset_next = __ballot_sync(kFull, ended) != 0u;
+    }
   }
 #ifdef MAPDN_PROFILE
   if (p.prof != nullptr && blockIdx.x == 0 && threadIdx.x == 0) for (int k = 0; k < 16; ++k) p.prof[k] = _acc[k];

@@ -142,6 +142,11 @@ struct Params {
   // MODE_STEP of a handle with history (or NULL): stacked rows [B, n_sgen, history * obs_dim], oldest frame first, zero
   // frames before the episode start (reference get_obs :303-315)
   double* obs_stacked;
+  // auto-reset step (mapdn_step_autoreset, or NULL): first observation of the new episode of every env that terminated in
+  // the step ([B, n_sgen, obs_dim]) and, with history, its stacked row ([B, n_sgen, history * obs_dim]); reset_ok above
+  // takes the reset outcome
+  double* reset_obs;
+  double* reset_obs_stacked;
 };
 
 // cold obs program entry: kind in the top 4 bits, node / sgen index in the low 28

@@ -120,27 +120,6 @@ __global__ void i64_to_double_kernel(long long n, const long long* __restrict__ 
   if (i < n) out[i] = static_cast<double>(in[i]);
 }
 
-// entry idx of get_obs() of env `env` from the state in HBM (reference :232-316), driven by the precomputed obs program
-__device__ __forceinline__ double obs_entry(const Params& p, int env, int idx) {
-  const size_t eN = static_cast<size_t>(env) * p.n_bus, eG = static_cast<size_t>(env) * p.n_sgen;
-  const unsigned src = __ldg(p.obs_src + idx);   // cold copy of the obs program (kind | node)
-  const int kind = static_cast<int>(src >> 28), ix = static_cast<int>(src & 0x0FFFFFFFu);
-  // node id -> bus id (npq = slack)
-  auto bus = [&](int i) { return (i == p.npq) ? p.slack_bus : __ldg(p.bus_of_node + i); };
-  double v = 0.0;
-  if (kind == OBS_P || kind == OBS_Q) {
-    v = (kind == OBS_P) ? p.res_p[eN + bus(ix)] : p.res_q[eN + bus(ix)];
-    for (int t = __ldg(p.obs_xptr + idx), te = __ldg(p.obs_xptr + idx + 1); t < te; ++t) {
-      const int sg = __ldg(p.obs_xidx + t);
-      v += (kind == OBS_P) ? p.cur_pv[eG + sg] : p.cur_q[eG + sg];
-    }
-  } else if (kind == OBS_PV) v = p.cur_pv[eG + ix];
-  else if (kind == OBS_QSG) v = p.cur_q[eG + ix];
-  else if (kind == OBS_VM) v = p.res_vm[eN + bus(ix)];
-  else if (kind == OBS_VA) v = p.res_va[eN + bus(ix)];
-  return v;
-}
-
 __global__ void get_obs_kernel(const __grid_constant__ Params p) {
   const int tot = p.n_sgen * p.obs_dim;
   const long long gid = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
@@ -221,7 +200,7 @@ struct mapdn_env {
   Params base{};                       // static + state pointers; io fields filled per call
   std::vector<void*> allocs;           // everything cudaMalloc'ed
   int G = 8, threads = 128, epb = 16, smem = 0, helper_threads = 32;
-  int max_blocks_step[2][2] = {};      // persistent grid of the MODE_STEP instantiations [observation history][tester records]
+  int max_blocks_step[2][2][2] = {};   // persistent grid of the MODE_STEP instantiations [auto-reset][observation history][tester records]
   bool dense = false;                  // meshed net: dense-LU fallback solver
   long long launches = 0;
   // Ybus pieces kept for the test hook
@@ -269,10 +248,11 @@ using KernelFn = void (*)(const Params);
 constexpr int kHelperPairsPerWarp = 256;   // Box-Muller pairs of a CTA round per helper warp
 
 template <int G, bool DENSE>
-KernelFn kernel_for_mode(int mode, bool record, bool hist) {
+KernelFn kernel_for_mode(int mode, bool record, bool hist, bool autoreset) {
   switch (mode) {
     case MODE_SOLVE: return env_kernel<G, MODE_SOLVE, DENSE>;
     case MODE_STEP:
+      if (autoreset) return hist ? env_kernel<G, MODE_STEP, DENSE, false, true, true> : env_kernel<G, MODE_STEP, DENSE, false, false, true>;
       if (hist) return record ? env_kernel<G, MODE_STEP, DENSE, true, true> : env_kernel<G, MODE_STEP, DENSE, false, true>;
       return record ? env_kernel<G, MODE_STEP, DENSE, true> : env_kernel<G, MODE_STEP, DENSE>;
     case MODE_DROOP: return env_kernel<G, MODE_DROOP, DENSE>;
@@ -281,16 +261,17 @@ KernelFn kernel_for_mode(int mode, bool record, bool hist) {
 }
 
 // record: the MODE_STEP instantiation that also writes the tester record rows (mapdn_step_record); hist: the one that
-// also records observation frames (handles with history)
-KernelFn kernel_for(int G, int mode, bool dense = false, bool record = false, bool hist = false) {
-  if (dense) return kernel_for_mode<32, true>(mode, record, hist);
+// also records observation frames (handles with history); autoreset: the one that also resets the envs that terminated
+// (mapdn_step_autoreset, never with record)
+KernelFn kernel_for(int G, int mode, bool dense = false, bool record = false, bool hist = false, bool autoreset = false) {
+  if (dense) return kernel_for_mode<32, true>(mode, record, hist, autoreset);
   switch (G) {
-    case 4: return kernel_for_mode<4, false>(mode, record, hist);
-    case 8: return kernel_for_mode<8, false>(mode, record, hist);
-    case 16: return kernel_for_mode<16, false>(mode, record, hist);
-    case 64: return kernel_for_mode<64, false>(mode, record, hist);
-    case 128: return kernel_for_mode<128, false>(mode, record, hist);
-    default: return kernel_for_mode<32, false>(mode, record, hist);
+    case 4: return kernel_for_mode<4, false>(mode, record, hist, autoreset);
+    case 8: return kernel_for_mode<8, false>(mode, record, hist, autoreset);
+    case 16: return kernel_for_mode<16, false>(mode, record, hist, autoreset);
+    case 64: return kernel_for_mode<64, false>(mode, record, hist, autoreset);
+    case 128: return kernel_for_mode<128, false>(mode, record, hist, autoreset);
+    default: return kernel_for_mode<32, false>(mode, record, hist, autoreset);
   }
 }
 
@@ -313,12 +294,12 @@ int env_stride2_for(int npq, int ng, int nl, int G, bool stage_rec) {
   return stride;
 }
 
-mapdn_status launch_env_kernel(mapdn_env* e, int mode, Params& p, cudaStream_t st) {
+mapdn_status launch_env_kernel(mapdn_env* e, int mode, Params& p, cudaStream_t st, bool autoreset = false) {
   const bool record = mode == MODE_STEP && p.record != nullptr;
   const bool hist = mode == MODE_STEP && p.history > 1;      // every step of a handle with history records its frame
-  KernelFn fn = kernel_for(e->G, mode, e->dense, record, hist);
+  KernelFn fn = kernel_for(e->G, mode, e->dense, record, hist, autoreset);
   const int needed = (p.nb + e->epb - 1) / e->epb;
-  int grid = std::min(needed, std::max(1, e->max_blocks_step[hist][record]));
+  int grid = std::min(needed, std::max(1, e->max_blocks_step[autoreset][hist][record]));
   const int rounds = (needed + grid - 1) / grid;
   grid = (needed + rounds - 1) / rounds;       // balance the persistent loop
 #ifdef MAPDN_PROFILE
@@ -353,15 +334,19 @@ mapdn_status launch_env_kernel(mapdn_env* e, int mode, Params& p, cudaStream_t s
 
 constexpr auto nothing = [](cudaStream_t) { return MAPDN_OK; };   // before / after of a step that needs neither
 
-// The MODE_STEP launch behind the seven mapdn_step* entry points, after each has checked its own pointers: refuses a
+// Outputs of the reset that mapdn_step_autoreset runs after the step (any may be NULL)
+struct AutoReset { double* obs; double* obs_stacked; uint8_t* ok; };
+
+// The MODE_STEP launch behind the eight mapdn_step* entry points, after each has checked its own pointers: refuses a
 // handle without a profile store, then runs on the handle's device. The kernel reads the actions from and writes its
 // outputs to the given buffers (info / obs / record may be NULL; obs holds floats when obs_f32). before(st) runs ahead of
-// the launch and may refuse the call or enqueue what the kernel reads; after(st) enqueues what follows the kernel.
+// the launch and may refuse the call or enqueue what the kernel reads; after(st) enqueues what follows the kernel. With
+// `autoreset`, the launch also resets the envs that terminate in the step.
 template <class Before, class After>
 mapdn_status step(mapdn_env* e, const double* actions, int32_t add_noise, double* reward, uint8_t* term, double* info,
                   void* obs, bool obs_f32, void* stream, Before before, After after, int obs_skip_off = -1,
                   int obs_compact_len = 0, double* record = nullptr, int64_t record_stride = 0,
-                  double* obs_stacked = nullptr) {
+                  double* obs_stacked = nullptr, const AutoReset* autoreset = nullptr) {
   if (!e->base.prof_pv) return fail(MAPDN_ERR_INVALID, "handle was created without a profile store");
   MAPDN_ON_DEVICE(e->device);
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -372,7 +357,8 @@ mapdn_status step(mapdn_env* e, const double* actions, int32_t add_noise, double
   p.obs = obs_f32 ? nullptr : static_cast<double*>(obs); p.obs32 = obs_f32 ? static_cast<float*>(obs) : nullptr;
   p.obs_skip_off = obs_skip_off; p.obs_compact_len = obs_compact_len; p.record = record; p.record_stride = record_stride;
   p.obs_stacked = obs_stacked;
-  s = launch_env_kernel(e, MODE_STEP, p, st);
+  if (autoreset) { p.reset_obs = autoreset->obs; p.reset_obs_stacked = autoreset->obs_stacked; p.reset_ok = autoreset->ok; }
+  s = launch_env_kernel(e, MODE_STEP, p, st, autoreset != nullptr);
   return s != MAPDN_OK ? s : after(st);
 }
 
@@ -1251,14 +1237,15 @@ std::vector<double> first_iteration_factors(const Forest& f, const HotBlob& hot,
   return ft;
 }
 
-// The shared-memory attribute of the seven kernel instantiations the handle launches, and the persistent grid of the four
+// The shared-memory attribute of the nine kernel instantiations the handle launches, and the persistent grid of the six
 // step variants (needs G, threads, helper_threads, smem and dense of the handle)
 mapdn_status size_kernels(mapdn_env* e, const cudaDeviceProp& dp) {
-  struct Variant { int mode; bool record, hist; };
-  const Variant variants[7] = {{MODE_STEP, false, false}, {MODE_STEP, true, false}, {MODE_STEP, false, true}, {MODE_STEP, true, true},
-                               {MODE_SOLVE, false, false}, {MODE_RESET, false, false}, {MODE_DROOP, false, false}};
-  for (const Variant& v : variants) {       // the plain step first: it bounds the grids of the other three
-    KernelFn fn = kernel_for(e->G, v.mode, e->dense, v.record, v.hist);
+  struct Variant { int mode; bool record, hist, autoreset; };
+  const Variant variants[9] = {{MODE_STEP, false, false, false}, {MODE_STEP, true, false, false}, {MODE_STEP, false, true, false},
+                               {MODE_STEP, true, true, false}, {MODE_STEP, false, false, true}, {MODE_STEP, false, true, true},
+                               {MODE_SOLVE, false, false, false}, {MODE_RESET, false, false, false}, {MODE_DROOP, false, false, false}};
+  for (const Variant& v : variants) {       // the plain step first: it bounds the grids of the other five
+    KernelFn fn = kernel_for(e->G, v.mode, e->dense, v.record, v.hist, v.autoreset);
     // the attribute belongs to the function, not to the handle: always allow the device maximum, so that creating a
     // second handle with a smaller footprint cannot break the launches of the first
     cudaFuncAttributes fa{};
@@ -1271,10 +1258,10 @@ mapdn_status size_kernels(mapdn_env* e, const cudaDeviceProp& dp) {
     MAPDN_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, e->threads + e->helper_threads, e->smem));
     int blocks = std::max(1, per_sm) * dp.multiProcessorCount;
     if (e->dense) blocks = std::min(blocks, 2 * dp.multiProcessorCount);   // bounds the dense workspace
-    // the record and history instantiations hold more registers: each persistent grid is sized by its own occupancy
-    // (never larger than the plain step's)
-    if (v.record || v.hist) blocks = std::min(blocks, e->max_blocks_step[0][0]);
-    e->max_blocks_step[v.hist][v.record] = blocks;
+    // the record, history and auto-reset instantiations hold more registers: each persistent grid is sized by its own
+    // occupancy (never larger than the plain step's)
+    if (v.record || v.hist || v.autoreset) blocks = std::min(blocks, e->max_blocks_step[0][0][0]);
+    e->max_blocks_step[v.autoreset][v.hist][v.record] = blocks;
   }
   return MAPDN_OK;
 }
@@ -1381,7 +1368,7 @@ mapdn_status upload_plan(mapdn_env* e, const mapdn_net_desc& net, const mapdn_pr
   if (f.meshed) {
     const size_t m = 2 * static_cast<size_t>(npq);
     P.dense_stride = static_cast<int>(m * (m + 1));
-    const size_t groups = static_cast<size_t>(e->max_blocks_step[0][0]) * e->epb;       // one slice per resident env group
+    const size_t groups = static_cast<size_t>(e->max_blocks_step[0][0][0]) * e->epb;       // one slice per resident env group
     MAPDN_TRY(dev_alloc(e, groups * P.dense_stride, &P.dense_ws));
   }
   // staging for the *_host entry points
@@ -1545,6 +1532,17 @@ mapdn_status mapdn_step_stacked(mapdn_env* e, const double* actions_dev, int32_t
   if (record_dev && record_stride < record_row_len(e)) return fail(MAPDN_ERR_INVALID, "record_stride shorter than a record row");
   return step(e, actions_dev, add_noise, reward_dev, terminated_dev, info_dev, obs_dev, false, stream, nothing, nothing,
               -1, 0, record_dev, record_stride, obs_stacked_dev);
+}
+
+mapdn_status mapdn_step_autoreset(mapdn_env* e, const double* actions_dev, int32_t add_noise, double* reward_dev,
+                                  uint8_t* terminated_dev, double* info_dev, double* obs_dev, double* obs_stacked_dev,
+                                  double* reset_obs_dev, double* reset_obs_stacked_dev, uint8_t* reset_ok_dev, void* stream) {
+  if (!e || !actions_dev || !reward_dev || !terminated_dev) return fail(MAPDN_ERR_INVALID, "null argument");
+  if (e->base.history <= 1 && (obs_stacked_dev || reset_obs_stacked_dev))
+    return fail(MAPDN_ERR_INVALID, "handle has no observation history (mapdn_set_history)");
+  const AutoReset ar{reset_obs_dev, reset_obs_stacked_dev, reset_ok_dev};
+  return step(e, actions_dev, add_noise, reward_dev, terminated_dev, info_dev, obs_dev, false, stream, nothing, nothing,
+              -1, 0, nullptr, 0, obs_stacked_dev, &ar);
 }
 
 mapdn_status mapdn_get_obs_stacked(mapdn_env* e, double* obs_stacked_dev, void* stream) {

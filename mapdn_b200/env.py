@@ -210,6 +210,32 @@ class BatchedVoltageControl:
             _capi.check(st)
         return self.reward, self.terminated, self.info
 
+    def step_autoreset(self, actions: torch.Tensor, add_noise: bool = True):
+        """:meth:`step` in which every env that terminates starts its next episode in the same launch
+        (``mapdn_step_autoreset``). Returns (reward, terminated, info) like :meth:`step`; ``self.obs`` /
+        ``self.obs_stacked`` hold the observation after the step (the terminal one of an env that ended). For the envs
+        with ``terminated = 1``, ``self.reset_obs`` (and ``self.reset_obs_stacked`` with ``history > 1``) hold the first
+        observation of the new episode and ``self.reset_ok`` the reset outcome, as :meth:`reset` with
+        ``mask=terminated`` would give them; the rows of the other envs are not written. No host sync.
+
+        So after this call ``self.obs`` / ``self.obs_stacked`` are not the current state's observation for the envs that
+        ended (``get_obs()`` / ``get_obs_stacked()`` are): a caller that resumes later keeps
+        ``torch.where(terminated, reset_obs, obs)`` as its current observation."""
+        if (actions.dtype is not torch.float64 or tuple(actions.shape) != self._act_shape or actions.device != self.device
+                or not actions.is_contiguous()):
+            self._chk(actions, self._act_shape, name="actions")
+        if getattr(self, "reset_obs", None) is None:
+            self.reset_obs = torch.zeros_like(self.obs)
+            self.reset_obs_stacked = torch.zeros_like(self.obs_stacked) if self.history > 1 else self.reset_obs
+        hist = self.history > 1
+        st = self._L.mapdn_step_autoreset(self._h, actions.data_ptr(), int(add_noise), self._p_reward, self._p_term,
+                                          self._p_info, self._p_obs, self.obs_stacked.data_ptr() if hist else None,
+                                          self.reset_obs.data_ptr(), self.reset_obs_stacked.data_ptr() if hist else None,
+                                          self.reset_ok.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream)
+        if st:
+            _capi.check(st)
+        return self.reward, self.terminated, self.info
+
     # host-buffer path (what a CPU-side caller such as the reference trainer pays end to end)
     def _host_buffers(self):
         if self._host is None:

@@ -148,6 +148,11 @@ def learner_obs(env) -> torch.Tensor:
     return env.obs_stacked if getattr(env, "history", 1) > 1 else env.obs
 
 
+def learner_reset_obs(env) -> torch.Tensor:
+    """:func:`learner_obs` of the new episodes that ``env.step_autoreset`` started (rows of the terminated envs)."""
+    return env.reset_obs_stacked if getattr(env, "history", 1) > 1 else env.reset_obs
+
+
 class BatchedMarlRunner:
     """``Model.train_process`` / ``Model.evaluation`` over B lock-step envs (see module docstring).
 
@@ -178,12 +183,16 @@ class BatchedMarlRunner:
         info_sum = torch.zeros(len(INFO_KEYS), dtype=torch.float64, device=env.device)
         reward_sum = torch.zeros((), dtype=torch.float64, device=env.device)
         n_steps = 0
+        # an env whose class has auto-reset re-draws the envs that terminate inside the step launch; the others (and
+        # wrappers that forward attributes, which may hook step / reset) get a masked reset
+        autoreset = callable(getattr(type(env), "step_autoreset", None))
+        step = env.step_autoreset if autoreset else env.step
         for t in range(args.max_steps):
             action, action_pol, log_prob_a, _, hid = net.get_actions(state, status="train", exploration=True,
                                                                      actions_avail=self._avail, target=False,
                                                                      last_hid=last_hid)
             value = net.value(state, action_pol)
-            reward, done, info = env.step(self._translate(action))
+            reward, done, info = step(self._translate(action))
             next_state = learner_obs(env).to(torch.float32).clone()
             _, next_action_pol, _, _, _ = net.get_actions(next_state, status="train", exploration=True,
                                                           actions_avail=self._avail, target=False, last_hid=hid)
@@ -203,9 +212,11 @@ class BatchedMarlRunner:
             if self.update_fn is not None:
                 self.update_fn(self, stat)
             # envs that ended early (divergence) start a new episode right away; the others carry on
-            env.reset(mask=done, want_state=False)
+            if not autoreset:
+                env.reset(mask=done, want_state=False)
+            first = learner_reset_obs(env) if autoreset else learner_obs(env)
             keep = (1.0 - done_f)[:, :, None]
-            state = torch.where(done.bool()[:, None, None], learner_obs(env).to(torch.float32), next_state)
+            state = torch.where(done.bool()[:, None, None], first.to(torch.float32), next_state)
             last_hid = hid.detach() * keep
         self.episodes += B
         denom = float(n_steps * B)

@@ -61,7 +61,8 @@ class DeviceReplayBuffer:
 class BatchedRollout:
     """Runs ``policy(obs[B, n_agents, obs_dim] fp32) -> raw actions [B, n_agents]`` on a
     :class:`~mapdn_b200.env.BatchedVoltageControl`, with the reference's action translation and
-    episode handling (terminated envs are re-drawn on the device, no host sync)."""
+    episode handling (terminated envs are re-drawn on the device, no host sync). Successive :meth:`run` calls continue
+    the same episodes: each starts from the observations the previous one returned."""
 
     def __init__(self, env, policy: Callable[[torch.Tensor], torch.Tensor], buffer: Optional[DeviceReplayBuffer] = None,
                  keep_returns: int = 1 << 16):
@@ -75,6 +76,9 @@ class BatchedRollout:
         self._ret_sum = torch.zeros((), dtype=torch.float64, device=env.device)
         self.info_sum = torch.zeros(env.batch, len(env.info[0]), dtype=torch.float64, device=env.device)
         self._started = False
+        # the observation every env's next step acts on. With auto-reset the env's own `obs` holds the terminal observation
+        # of an env that just ended (its new episode's first one is in `reset_obs`), so the rollout keeps its own.
+        self._obs = None
 
     @torch.no_grad()
     def run(self, n_steps: int, add_noise: bool = True):
@@ -82,11 +86,16 @@ class BatchedRollout:
         if not self._started:
             env.reset()
             self._started = True
-        obs = env.obs.clone()
+            self._obs = env.obs.clone()
+        obs = self._obs
+        # an env whose class has auto-reset re-draws the envs that terminate inside the step launch; the others (and
+        # wrappers that forward attributes, which may hook step / reset) get a masked reset
+        autoreset = callable(getattr(type(env), "step_autoreset", None))
+        step = env.step_autoreset if autoreset else env.step
         for _ in range(n_steps):
             raw = self.policy(obs.to(torch.float32))
             act = translate_action(raw.reshape(env.batch, env.n_agents), self.scale, self.bias).contiguous()
-            reward, done, info = env.step(act, add_noise=add_noise)
+            reward, done, info = step(act, add_noise=add_noise)
             next_obs = env.obs.clone()
             if self.buffer is not None:
                 self.buffer.add_batch(obs, raw.reshape(env.batch, env.n_agents), reward, next_obs, done)
@@ -101,9 +110,11 @@ class BatchedRollout:
             self._ret_sum += (self.episode_return * d).sum()
             self._ret_n += d.sum()
             self.episode_return = torch.where(done.bool(), torch.zeros_like(self.episode_return), self.episode_return)
-            env.reset(mask=done, want_state=False)                      # masked, stream-ordered: only terminated envs are re-drawn
-            obs = torch.where(done.bool()[:, None, None], env.obs, next_obs)
-        return obs
+            if not autoreset:
+                env.reset(mask=done, want_state=False)                  # masked, stream-ordered: only terminated envs are re-drawn
+            obs = torch.where(done.bool()[:, None, None], env.reset_obs if autoreset else env.obs, next_obs)
+        self._obs = obs
+        return obs.clone()
 
     def completed_episode_returns(self) -> torch.Tensor:
         """Returns of the episodes that ended so far - the last ``keep_returns`` of them (one host sync)."""
