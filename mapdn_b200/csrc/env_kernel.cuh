@@ -286,6 +286,8 @@ struct Slab {
   double* pv;       // sgen.p_mw   [n_sgen]
   double* q;        // sgen.q_mvar [n_sgen]
   double* scratch;  // [n_sgen + 2 n_load]
+  double* red;      // in scratch: the per-warp partials of the multi-warp group reductions
+  double* stage;    // in scratch: the staged loads, when they do not fit the node records
   __device__ __forceinline__ double2* node(int i) const { return nodes + i * kNodeArrays2; }
 };
 
@@ -759,15 +761,16 @@ __device__ __forceinline__ double clip_q(double a, double pv, double smax) {
   return sqrt(smax * smax - pv * pv) * a;
 }
 
-// Stacked observation row of one env (reference get_obs :303-315): agent a's block k (oldest first) is frame
-// f - (history - 1) + k; a frame with a negative index (before the episode start) is zero, the others come from the ring.
-// newest(i) gives entry i of frame f when the caller holds it elsewhere (the step kernel: its shared-memory slab). Lanes
-// lane, lane + nlanes, ... store consecutive 16-byte pieces (even obs_dim), else single entries.
+// Stacked observation row of one env (reference get_obs :303-315) into its row of dst (Params::obs_stacked, or
+// Params::reset_obs_stacked after an auto-reset): agent a's block k (oldest first) is frame f - (history - 1) + k; a frame
+// with a negative index (before the episode start) is zero, the others come from the ring. newest(i) gives entry i of frame
+// f when the caller holds it elsewhere (the step kernel: its shared-memory slab). Lanes lane, lane + nlanes, ... store
+// consecutive 16-byte pieces (even obs_dim), else single entries.
 template <class Newest>
-__device__ __forceinline__ void write_stacked_row(const Params& p, int env, int f, int lane, int nlanes, Newest newest) {
+__device__ __forceinline__ void write_stacked_row(const Params& p, double* dst, int env, int f, int lane, int nlanes, Newest newest) {
   const int od = p.obs_dim, H = p.history, tot = p.n_sgen * od, blk = H * od;
   const double* ring = p.hist + static_cast<size_t>(env) * H * tot;
-  double* o = p.obs_stacked + static_cast<size_t>(env) * p.n_sgen * blk;
+  double* o = dst + static_cast<size_t>(env) * p.n_sgen * blk;
   auto entry = [&](int e, double* v, int n) {        // n consecutive entries from e (inside one frame block)
     const int a = e / blk, r = e - a * blk, k = r / od, j = r - k * od;
     const int fk = f - (H - 1) + k, i = a * od + j;
@@ -779,7 +782,7 @@ __device__ __forceinline__ void write_stacked_row(const Params& p, int env, int 
     else v[0] = *src;
   };
   const int row = p.n_sgen * blk;
-  if ((od & 1) == 0 && (reinterpret_cast<uintptr_t>(p.obs_stacked) & 15) == 0) {
+  if ((od & 1) == 0 && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
     for (int c = lane; c < row / 2; c += nlanes) {
       double v[2];
       entry(2 * c, v, 2);
@@ -788,6 +791,15 @@ __device__ __forceinline__ void write_stacked_row(const Params& p, int env, int 
   } else {
     for (int e = lane; e < row; e += nlanes) { double v[1]; entry(e, v, 1); o[e] = v[0]; }
   }
+}
+
+// Frame 0 of a new episode into slot 0 of the env's ring, entry i = frame0(i), lanes lane, lane + nlanes, ... Its stacked
+// row is write_stacked_row at f = 0: history - 1 zero frames, then frame 0.
+template <class Frame0>
+__device__ __forceinline__ void write_frame0(const Params& p, int env, int lane, int nlanes, Frame0 frame0) {
+  const int tot = p.n_sgen * p.obs_dim;
+  double* fr = p.hist + static_cast<size_t>(env) * p.history * tot;
+  for (int i = lane; i < tot; i += nlanes) fr[i] = frame0(i);
 }
 
 // entry idx of get_obs() of env `env` from the state in HBM (reference :232-316), driven by the precomputed obs program
@@ -811,11 +823,481 @@ __device__ __forceinline__ double obs_entry(const Params& p, int env, int idx) {
   return v;
 }
 
+// ------------------------------------------------------------------------------------------
+// Stages of env_kernel's persistent loop, in the order the loop runs them. Each works on the env of one G-lane group in
+// one pass of the loop; the mode is the pass's (MODE_RESET in the auto-reset pass of a MODE_STEP launch).
+// ------------------------------------------------------------------------------------------
+struct EnvPass {
+  int mode;
+  bool auto_pass;          // the auto-reset pass of a MODE_STEP launch
+  int env;                 // groups beyond the batch work on env nb - 1 and store nothing (valid = false)
+  bool valid;              // the group stores its results: in the batch and selected
+  size_t eL, eG, eN;       // first entry of the env's rows: loads, sgens, buses
+  int gidx, gl;            // the group in the CTA, the lane in the group
+  int npq, n, nl, ng;      // the kernel's sizes, read once: a reload after a barrier is another load
+};
+
+// Per-env sums and maxima of a step's results (reference _calc_reward :584-596, :610), reduced over the group for the
+// reward and the info; sum_pl is also the droop baseline's loss
+struct StepStats {
+  double cnt_lo = 0, cnt_hi = 0, sum_dev = 0, sum_v = 0, max_drop = 0, max_rise = 0, sum_bar = 0, sum_pl = 0;
+  double sum_q_eff = 0, sum_q_try = 0;
+};
+
+// MODE_STEP helper warps: next profile row of every env of this round (reference _set_demand_and_pv :491-513: t =
+// self.steps before the increment) + |N(0,1)| * std noise in Box-Muller pairs (2m, 2m+1) over the elements
+// [pv | load_p | load_q]; new pv goes to the env's scratch (for the obs), loads straight to HBM. Two dependent global round
+// trips in total: (A) the per-env scalars of the whole round -> shared memory, (B) the profile values, four work items per
+// thread in flight, addresses selected without branches. The helpers meet the solver warps only at the named barriers 1
+// (the solvers have read the current rows) and 2 (the new pv is in shared memory).
+__device__ __forceinline__ void helper_draw_rows(const Params& p, unsigned char* smem, int base, int epb, int n_solver_threads,
+                                                 int n_helper_threads, uint32_t k0, uint32_t k1, int ng, int nl, int hl_bytes) {
+  const int n_elem = ng + 2 * nl, n_pair = (n_elem + 1) / 2, n_work = epb * n_pair;
+  const int ht = threadIdx.x - n_solver_threads, T = n_helper_threads;
+  int4* hs = reinterpret_cast<int4*>(smem + p.helper_off);     // per env: (row lo, row hi, steps, episode)
+#ifdef MAPDN_HOST_EMU
+  emu::bar_sync(15, T);
+#else
+  asm volatile("bar.sync 15, %0;" ::"r"(T) : "memory");     // helper threads only: the previous round's reads of hs are done
+#endif
+  for (int e = ht; e < epb; e += T) {
+    const int env_h = base + e;
+    int4 v = make_int4(0, 0, 0, 0);
+    if (env_h < p.nb) {
+      const int steps_h = p.steps[env_h];
+      long long nrow = p.start_row[env_h] + steps_h;
+      if (nrow > p.n_rows - 1) nrow = p.n_rows - 1;
+      v = make_int4(static_cast<int>(nrow & 0xFFFFFFFFll), static_cast<int>(nrow >> 32), steps_h,
+                    static_cast<int>(p.episode[env_h]));
+    }
+    hs[e] = v;
+  }
+#ifdef MAPDN_HOST_EMU
+  emu::bar_sync(15, T);
+#else
+  asm volatile("bar.sync 15, %0;" ::"r"(T) : "memory");     // helper threads only
+#endif
+  named_bar_sync(1, blockDim.x);                   // the solvers have read the current rows
+  constexpr int U = 4;
+  for (int w0 = ht; w0 < n_work; w0 += U * T) {
+    double val[U][2], sd[U][2];
+    int e_[U], m_[U];
+    bool ok[U];
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int w = w0 + u * T;
+      ok[u] = w < n_work;
+      const int e = ok[u] ? w / n_pair : 0;
+      e_[u] = e; m_[u] = w - e * n_pair;
+      ok[u] = ok[u] && (base + e < p.nb);
+      const int4 sc = hs[e];
+      const long long nrow = (static_cast<long long>(sc.y) << 32) | static_cast<unsigned>(sc.x);
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        const int el = min(2 * m_[u] + k, n_elem - 1);          // an odd n_elem re-reads the last element (not stored)
+        const bool is_pv = el < ng, is_lp = el < ng + nl;
+        const int j = is_pv ? el : (is_lp ? el - ng : el - ng - nl);
+        const double* src = is_pv ? p.prof_pv + nrow * ng : (is_lp ? p.prof_lp + nrow * nl : p.prof_lq + nrow * nl);
+        const double* sds = is_pv ? p.pv_std : (is_lp ? p.lp_std : p.lq_std);
+        val[u][k] = ok[u] ? __ldg(src + j) : 0.0;
+        sd[u][k] = ok[u] ? __ldg(sds + j) : 0.0;
+      }
+    }
+    // one copy of Philox + log + sqrt + sincos (not four: the solver warps need the instruction cache); the work
+    // item is picked out of the registers with select chains
+#pragma unroll 1
+    for (int u = 0; u < U; ++u) {
+      bool oku = ok[0]; int e = e_[0], m = m_[0];
+      double va = val[0][0], vb = val[0][1], sa = sd[0][0], sb = sd[0][1];
+#pragma unroll
+      for (int q = 1; q < U; ++q)
+        if (u == q) { oku = ok[q]; e = e_[q]; m = m_[q]; va = val[q][0]; vb = val[q][1]; sa = sd[q][0]; sb = sd[q][1]; }
+      if (!oku) continue;
+      const int env_h = base + e;
+      const int4 sc = hs[e];
+      RngKey key_h{k0, k1, static_cast<uint32_t>(p.env_id_offset + env_h), static_cast<uint32_t>(sc.w) * 8u};
+      double z0 = 0.0, z1 = 0.0;
+      if (p.add_noise) half_normal_pair(key_h, static_cast<uint32_t>(sc.z), m, z0, z1);
+      double* pv_next = reinterpret_cast<double*>(reinterpret_cast<double2*>(smem + hl_bytes) +
+                                                   static_cast<size_t>(e) * p.env_stride2 + p.scratch_off2);
+      const size_t hL = static_cast<size_t>(env_h) * nl, hG = static_cast<size_t>(env_h) * ng;
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        const int el = 2 * m + k;
+        if (el >= n_elem) break;
+        const double v = (k == 0) ? va + sa * z0 : vb + sb * z1;
+        const bool is_pv = el < ng, is_lp = el < ng + nl;
+        double* dst = is_pv ? p.cur_pv + hG + el : (is_lp ? p.cur_pl + hL + (el - ng) : p.cur_ql + hL + (el - ng - nl));
+        *dst = v;
+        if (is_pv) pv_next[el] = v;
+      }
+    }
+  }
+  named_bar_arrive(2, blockDim.x);                 // new pv of every env is in shared memory
+}
+
+// MODE_RESET: the first profile row of the new episode, the caller's start (manual_reset :137-152) or one drawn with the
+// attempt's counter (:111-113, :381-398)
+__device__ __forceinline__ long long reset_start(const Params& p, const EnvPass& e, const RngKey& key, int attempt) {
+  int day, hour, interval;
+  if (!e.auto_pass && p.start_dhi != nullptr) {
+    day = p.start_dhi[e.env * 3 + 0]; hour = p.start_dhi[e.env * 3 + 1]; interval = p.start_dhi[e.env * 3 + 2];
+  } else {
+    const u32x4 r = philox4x32_10(0u, static_cast<uint32_t>(attempt), key.env, key.c3base + kStreamTime, key.k0, key.k1);
+    hour = static_cast<int>(__umulhi(r.x, 24u));
+    day = static_cast<int>(__umulhi(r.y, static_cast<uint32_t>(p.n_day_choices)));
+    interval = static_cast<int>(__umulhi(r.z, static_cast<uint32_t>(p.steps_per_hour)));
+  }
+  const long long start = interval + static_cast<long long>(hour) * p.steps_per_hour +
+                          static_cast<long long>(day) * 24 * p.steps_per_hour;          // :445
+  // a manual start outside the store is clamped to the last window that fits (the host shims validate and raise; the
+  // kernel only guarantees in-bounds reads)
+  return max(0ll, min(start, p.n_rows - 1 - p.episode_limit));
+}
+
+// Prologue of a round: element values -> sgen p/q and bus injections. MODE_DROOP loads the sgens in round 0 only (later
+// rounds only change q, in shared memory) and re-stages the loads every round (the Newton iteration overwrites the staging
+// area).
+template <int G>
+__device__ __forceinline__ void prologue(const Params& p, const Hot& h, const Slab& s, const EnvPass& e, const RngKey& key,
+                                         long long start, int attempt, int round, bool stage_rec, bool& hot_ready,
+                                         uint64_t* stage_bar) {
+  const int M = e.mode, gidx = e.gidx, gl = e.gl, npq = e.npq, nl = e.nl, ng = e.ng;
+  const bool valid = e.valid, auto_pass = e.auto_pass;
+  const size_t eL = e.eL, eG = e.eG;
+  double* v_last = s.scratch;
+  long long row = 0;
+  if (M == MODE_RESET) { row = start + 1; if (row > p.n_rows - 1) row = p.n_rows - 1; }   // t = steps = 1
+  const uint32_t c1 = kResetFlag | static_cast<uint32_t>(attempt);
+  // (1) coalesced, independent loads of the env's element values into shared memory
+  if (M != MODE_DROOP || round == 0) {
+#pragma unroll 4
+  for (int j = gl; j < ng; j += G) {
+    double pv, q;
+    if (M == MODE_SOLVE || M == MODE_DROOP) {
+      pv = p.in_pv[eG + j]; q = (M == MODE_SOLVE) ? p.in_q[eG + j] : 0.0;     // droop starts from q = 0 (:107)
+      if (M == MODE_DROOP) v_last[j] = 100.0;                                    // :123
+    } else if (M == MODE_STEP) {
+      pv = p.cur_pv[eG + j];
+      q = clip_q(p.actions[eG + j], pv, __ldg(p.s_max + j));             // :553
+    } else {
+      pv = __ldg(p.prof_pv + row * ng + j);
+      if (auto_pass || p.add_noise) pv += __ldg(p.pv_std + j) * half_normal(key, c1, j);   // :498
+      q = 0.0;
+      if (p.reset_action) {                                               // :120-122, :334-338
+        const u32x4 r = philox4x32_10(j, static_cast<uint32_t>(attempt), key.env, key.c3base + kStreamAction, key.k0, key.k1);
+        const double a = p.action_low + (p.action_high - p.action_low) * u53(r.x, r.y);
+        q = clip_q(a, pv, __ldg(p.s_max + j));
+      }
+      if (valid) p.cur_pv[eG + j] = pv;
+    }
+    s.pv[j] = pv; s.q[j] = q;
+  }
+  }
+  // Staged (scaled) load p / q, 2 n_load doubles: they normally live in the Newton fields of the node records (UP .. R = 12
+  // contiguous doubles per record), which are dead until the flat start overwrites them. Written once, instantiated for the
+  // two staging places (block-uniform choice): a branch per access inside the loops would cost time in every step.
+  auto stage_and_gather = [&](auto stg) {
+#pragma unroll 4
+    for (int l = gl; l < nl; l += G) {
+      double pl, ql;
+      if (M == MODE_SOLVE || M == MODE_DROOP) { pl = p.in_pl[eL + l]; ql = p.in_ql[eL + l]; }
+      else if (M == MODE_STEP) { pl = p.cur_pl[eL + l]; ql = p.cur_ql[eL + l]; }
+      else {
+        pl = __ldg(p.prof_lp + row * nl + l);
+        ql = __ldg(p.prof_lq + row * nl + l);
+        if (auto_pass || p.add_noise) {                                      // :503, :508
+          pl += __ldg(p.lp_std + l) * half_normal(key, c1, ng + l);
+          ql += __ldg(p.lq_std + l) * half_normal(key, c1, ng + nl + l);
+        }
+        if (valid) { p.cur_pl[eL + l] = pl; p.cur_ql[eL + l] = ql; }
+      }
+      const double sc = __ldg(p.lscale + l);
+      *stg(l) = pl * sc; *stg(nl + l) = ql * sc;
+    }
+    if (!hot_ready) { stage_hot_wait(stage_bar); hot_ready = true; }
+    grp_sync<G>(gidx);
+    // (2) A.1: PD/QD per bus, Sbus = -(PD + jQD)/baseMVA
+    for (int i = gl; i < npq; i += G) {
+      double pd = 0.0, qd = 0.0;
+#pragma unroll 1
+      for (int t = h.lptr[i], te = h.lptr[i + 1]; t < te; ++t) { const int l = h.lidx[t]; pd += *stg(l); qd += *stg(nl + l); }
+#pragma unroll 1
+      for (int t = h.sptr[i], te = h.sptr[i + 1]; t < te; ++t) {
+        const int g = h.sidx[t];
+        const double sc = __ldg(p.sscale + g);
+        pd -= s.pv[g] * sc; qd -= s.q[g] * sc;
+      }
+      s.node(i)[A_SP] = make_double2(-pd * p.inv_base, -qd * p.inv_base);
+    }
+  };
+  if (stage_rec) stage_and_gather([&](int k) -> double* { return s.base + (k / 12) * (2 * kNodeArrays2) + 2 * A_UP + (k % 12); });
+  else stage_and_gather([&](int k) -> double* { return s.stage + k; });
+  grp_sync<G>(gidx);
+  if (M == MODE_STEP) named_bar_arrive(1, blockDim.x);   // the current rows are consumed: the helper may overwrite them
+}
+
+// After the round loop: the divergence branch of a step (reference :188-196) falls back to the previous solution kept in
+// HBM; the solve's outcome per env; the slack injection (pfsoln, SURVEY A.5): S0 = V0 conj(Ybus[0,:] V) -> the sentinel
+// record's SP
+template <int G>
+__device__ __forceinline__ void fallback_and_slack(const Params& p, const Slab& s, const EnvPass& e, bool conv, int iters) {
+  const int M = e.mode, env = e.env, gidx = e.gidx, gl = e.gl, npq = e.npq;
+  const bool valid = e.valid;
+  const size_t eN = e.eN;
+  if (M == MODE_STEP && !conv) {
+    for (int i = gl; i < npq; i += G) {
+      const int b = __ldg(p.bus_of_node + i);
+      const double vm = p.res_vm[eN + b], va = p.res_va[eN + b];
+      double sn, cs;
+      sincos(va, &sn, &cs);
+      double2* nd = s.node(i);
+      nd[A_VV] = make_double2(vm, va);
+      nd[A_EF] = make_double2(vm * cs, vm * sn);
+      nd[A_SP] = make_double2(-p.res_p[eN + b] * p.inv_base, -p.res_q[eN + b] * p.inv_base);
+    }
+  }
+  grp_sync<G>(gidx);
+  const bool kExplicit = (M == MODE_SOLVE || M == MODE_DROOP);
+  if (M == MODE_RESET && valid && gl == 0 && p.reset_ok != nullptr) p.reset_ok[env] = conv ? 1 : 0;
+  if (!kExplicit && valid && gl == 0) p.nr_iters[env] = conv ? iters : p.max_iter;
+
+  const double vv = p.vm0 * p.vm0;
+  double P0 = p.ysl_g0 * vv, Q0 = -p.ysl_b0 * vv;
+  for (int k = 0; k < p.n_slack_adj; ++k) {
+    const int i = __ldg(p.sl_node + k);
+    const double g = __ldg(p.sl_y + 2 * k), b = __ldg(p.sl_y + 2 * k + 1);
+    const double2 vi = s.node(i)[A_EF];
+    const double cc = p.e0 * vi.x + p.f0 * vi.y, ss = p.f0 * vi.x - p.e0 * vi.y;   // V0 Vi cos/sin(t0 - ti)
+    P0 += g * cc + b * ss;
+    Q0 += g * ss - b * cc;
+  }
+  if (gl == 0) s.node(npq)[A_SP] = make_double2(P0, Q0);
+}
+
+// MODE_STEP: sgen.q_mvar after the step, the clipped action or the previous q on divergence (:189-196), then the next
+// profile row's sgen.p_mw that the helper warp has drawn meanwhile (Appendix B.3: the observation mixes this solve's bus
+// results with the NEXT row's PV).
+// RECORD: record row [pv | q | P_bus | Q_bus | vm | line loss] (the order of the reference tester's getters): exactly what
+// mapdn_get_field returns after this step. pv is already the next profile row (reference :199 runs before the tester's
+// getters); q is the effective one; a diverged env reports its previous results, read back from HBM (bus_results).
+template <int G, bool RECORD>
+__device__ __forceinline__ void effective_q_and_next_row(const Params& p, const Slab& s, const EnvPass& e, bool conv,
+                                                         bool write_res, double* rec, StepStats& st) {
+  const int M = e.mode, gidx = e.gidx, gl = e.gl, ng = e.ng;
+  const bool valid = e.valid;
+  const size_t eG = e.eG;
+  const double* next_row = s.scratch;
+  if (M == MODE_STEP) {
+    for (int j = gl; j < ng; j += G) {
+      const double q_try = s.q[j];
+      const double q_eff = conv ? q_try : p.cur_q[eG + j];
+      st.sum_q_try += fabs(q_try);
+      st.sum_q_eff += fabs(q_eff * __ldg(p.sscale + j));     // res_sgen.q_mvar = q * scaling (:604-605)
+      s.q[j] = q_eff;
+      if (write_res) p.cur_q[eG + j] = q_eff;
+    }
+  }
+  if (M == MODE_STEP) {
+    named_bar_sync(2, blockDim.x);
+    for (int j = gl; j < ng; j += G) s.pv[j] = next_row[j];
+    if constexpr (RECORD) {
+      if (valid)
+        for (int j = gl; j < ng; j += G) { rec[j] = s.pv[j]; rec[ng + j] = s.q[j]; }
+    }
+  }
+  grp_sync<G>(gidx);
+}
+
+// Bus and line results: res_bus columns per node (BP) and the "demand" columns of get_obs (OP = BP + sgens of the bus's
+// own zone); per-bus results (res_* of the env state, or the explicit outputs of MODE_SOLVE / MODE_DROOP), the voltage
+// statistics of a step (reference _calc_reward :584-596, :610) and the line losses
+template <int G, bool RECORD>
+__device__ __forceinline__ void bus_results(const Params& p, const Hot& h, const Slab& s, const EnvPass& e, bool conv,
+                                            bool write_res, double* rec, StepStats& st) {
+  const int M = e.mode, env = e.env, gidx = e.gidx, gl = e.gl, npq = e.npq, n = e.n, ng = e.ng;
+  const bool valid = e.valid;
+  const size_t eN = e.eN;
+  const bool kExplicit = (M == MODE_SOLVE || M == MODE_DROOP);
+  for (int i = gl; i <= npq; i += G) {
+    double2* nd = s.node(i);
+    const double2 sp = nd[A_SP];
+    double2 bp = make_double2(-sp.x * p.base_mva, -sp.y * p.base_mva);
+    if (p.has_shunt) {                   // warp-uniform; pandapower adds the bus shunts' p/q (x vm^2) to res_bus
+      const double2 ef = nd[A_EF];
+      const double v2 = ef.x * ef.x + ef.y * ef.y;
+      bp.x += __ldg(p.sh_g + i) * v2; bp.y -= __ldg(p.sh_b + i) * v2;
+    }
+    double2 op = bp;
+#pragma unroll 1
+    for (int t = h.xptr[i], te = h.xptr[i + 1]; t < te; ++t) { const int g = h.xidx[t]; op.x += s.pv[g]; op.y += s.q[g]; }
+    nd[A_BP] = bp; nd[A_OP] = op;
+  }
+  grp_sync<G>(gidx);
+  const double v_ref = 0.5 * (p.v_lower + p.v_upper);
+#pragma unroll 4
+  for (int b = gl; b < n; b += G) {
+    const double2* nd = s.node(h.node_of_bus[b]);
+    const double2 vv = nd[A_VV], bp = nd[A_BP];
+    const double v = vv.x, th = vv.y;
+    if (kExplicit) {
+      if (valid) {
+        if (p.out_vm) p.out_vm[eN + b] = v;
+        if (p.out_va) p.out_va[eN + b] = th * kRad2Deg;
+        if (p.out_p) p.out_p[eN + b] = bp.x;
+        if (p.out_q) p.out_q[eN + b] = bp.y;
+      }
+    } else {
+      if (write_res) {
+        p.res_vm[eN + b] = v; p.res_va[eN + b] = th; p.res_p[eN + b] = bp.x; p.res_q[eN + b] = bp.y;
+      }
+      if constexpr (RECORD) {         // consecutive lanes, consecutive buses: coalesced like the res_* stores
+        if (valid) {
+          rec[2 * ng + b] = conv ? bp.x : p.res_p[eN + b];
+          rec[2 * ng + n + b] = conv ? bp.y : p.res_q[eN + b];
+          rec[2 * ng + 2 * n + b] = v;                    // on divergence: reloaded from res_vm by fallback_and_slack
+        }
+      }
+      if (M == MODE_STEP) {
+        st.cnt_lo += (v < p.v_lower) ? 1.0 : 0.0;
+        st.cnt_hi += (v > p.v_upper) ? 1.0 : 0.0;
+        st.sum_dev += fabs(v - v_ref);
+        st.sum_v += v;
+        st.max_drop = fmax(st.max_drop, (v < p.v_lower) ? (p.v_lower - v) : 0.0);
+        st.max_rise = fmax(st.max_rise, (v > p.v_upper) ? (v - p.v_upper) : 0.0);
+        st.sum_bar += barrier_fn(p.barrier, v);
+      }
+    }
+  }
+  // line losses: res_line.pl_mw = Re(Sf + St) (SURVEY A.5), 4 static coefficients per line. The two tables are either
+  // part of the staged blob (LDS) or cold in global memory (read-only path): one block-uniform branch, two typed loops.
+  const size_t ePL = static_cast<size_t>(env) * p.n_line;
+  auto lines = [&](const ushort2* __restrict__ ln, const double2* __restrict__ lc) {
+#pragma unroll 4
+    for (int k = gl; k < p.n_line; k += G) {
+      const ushort2 ft = ln[k];
+      const double2 vf = s.node(ft.x)[A_EF], vt = s.node(ft.y)[A_EF];
+      const double cc = vf.x * vt.x + vf.y * vt.y, ss = vf.y * vt.x - vf.x * vt.y;
+      const double2 c01 = lc[2 * k], c23 = lc[2 * k + 1];
+      const double pl = c01.x * (vf.x * vf.x + vf.y * vf.y) + c01.y * (vt.x * vt.x + vt.y * vt.y) + c23.x * cc + c23.y * ss;
+      st.sum_pl += pl;
+      if (kExplicit) { if (valid && p.out_pl) p.out_pl[ePL + k] = pl; }
+      else if (write_res) p.res_pl[ePL + k] = pl;
+      if constexpr (RECORD) {
+        if (valid) rec[2 * ng + 3 * n + k] = conv ? pl : p.res_pl[ePL + k];
+      }
+    }
+  };
+  const HotLayout& hl = p.hot_layout;
+  if (h.in_blob) lines(reinterpret_cast<const ushort2*>(h.blob + hl.line_nodes), reinterpret_cast<const double2*>(h.blob + hl.line_c));
+  else lines(reinterpret_cast<const ushort2*>(p.line_nodes), reinterpret_cast<const double2*>(p.line_c));
+}
+
+// MODE_SOLVE / MODE_DROOP: the explicit outputs besides the bus and line results
+template <int G>
+__device__ __forceinline__ void explicit_outputs(const Params& p, const Slab& s, const EnvPass& e, bool conv, int iters,
+                                                 int dr_iters, double sum_pl) {
+  const int M = e.mode, env = e.env, gidx = e.gidx, gl = e.gl, ng = e.ng;
+  const bool valid = e.valid;
+  const size_t eG = e.eG;
+  if (M == MODE_DROOP) {
+    double tot[1] = {sum_pl};
+    const bool no_max[1] = {false};
+    grp_reduce<G, 1>(gidx, gl, tot, no_max, s.red);
+    if (valid) {
+      for (int j = gl; j < ng; j += G) p.droop_q_out[eG + j] = s.q[j];
+      if (gl == 0) { p.droop_loss_out[env] = tot[0]; p.out_iters[env] = dr_iters; }
+    }
+  }
+  if (valid && gl == 0) {
+    if (M == MODE_SOLVE && p.out_iters) p.out_iters[env] = conv ? iters : p.max_iter;
+    if (p.out_conv) p.out_conv[env] = conv ? 1 : 0;
+  }
+  grp_sync<G>(gidx);
+}
+
+// MODE_RESET: the new episode's sgen q and counters (reference reset() :96-135). A reset whose kMaxResetAttempts draws all
+// diverged keeps only the env's previous power-flow results (res_*, see write_res) and reports it (reset_ok); cur_* hold
+// the last draw and the counters, start_row and episode start the new episode as after a converged reset.
+template <int G>
+__device__ __forceinline__ void reset_bookkeeping(const Params& p, const Slab& s, const EnvPass& e, long long start) {
+  const int env = e.env, gl = e.gl, ng = e.ng;
+  const bool valid = e.valid;
+  const size_t eG = e.eG;
+  for (int j = gl; j < ng; j += G) if (valid) p.cur_q[eG + j] = s.q[j];
+  if (valid && gl == 0) {
+    p.steps[env] = 1;                         // :100
+    p.sum_rewards[env] = 0.0;                 // :101
+    p.start_row[env] = start;
+    p.episode[env] = p.episode[env] + 1u;
+  }
+}
+
+// HIST, step pass: frame f = steps - 1 of this step into its ring slot, through the padded program whatever layout
+// (compact, fp32, none) the caller's observations take; then the stacked row, whose newest frame comes straight from the
+// slab
+template <int G>
+__device__ __forceinline__ void step_history(const Params& p, const Hot& h, const Slab& s, const EnvPass& e, int steps_old) {
+  if (!e.valid) return;
+  const int env = e.env, gl = e.gl;
+  const int f = steps_old, tot = e.ng * p.obs_dim;
+  const uint16_t* prog = h.in_blob ? reinterpret_cast<const uint16_t*>(h.blob + p.hot_layout.obs_off) : p.obs_off;
+  double* fr = p.hist + (static_cast<size_t>(env) * p.history + f % p.history) * tot;
+  if ((tot & 1) == 0) {
+    for (int c = gl; c < tot / 2; c += G)
+      *reinterpret_cast<double2*>(fr + 2 * c) = make_double2(s.base[prog[2 * c]], s.base[prog[2 * c + 1]]);
+  } else {
+    for (int i = gl; i < tot; i += G) fr[i] = s.base[prog[i]];
+  }
+  if (p.obs_stacked != nullptr) write_stacked_row(p, p.obs_stacked, env, f, gl, G, [&](int i) { return s.base[prog[i]]; });
+}
+
+// HIST, auto-reset pass: frame 0 of the new episode and its stacked row, the values reset_frame_kernel and
+// obs_stacked_kernel give after a reset launch. Frame 0 comes from the slab through the padded program when the reset
+// converged (the state in HBM holds the same values), else from the state in HBM (a reset whose draws all diverged keeps
+// the old res_*, which its slab does not hold; the group's stores must be visible to every lane of the group first). The
+// stacked row takes frame 0 from the slab as well when the reset converged, else it reads it back from ring slot 0 (like
+// obs_stacked_kernel), so that obs_entry is expanded once. Every lane of the group (of the warp, for G <= 32) reaches both
+// group barriers: the pass's entry is uniform.
+template <int G>
+__device__ __forceinline__ void reset_history(const Params& p, const Hot& h, const Slab& s, const EnvPass& e, bool conv) {
+  const int env = e.env, gl = e.gl;
+  const uint16_t* prog = h.in_blob ? reinterpret_cast<const uint16_t*>(h.blob + p.hot_layout.obs_off) : p.obs_off;
+  grp_sync<G>(e.gidx);
+  if (e.valid) write_frame0(p, env, gl, G, [&](int i) { return conv ? s.base[prog[i]] : obs_entry(p, env, i); });
+  grp_sync<G>(e.gidx);       // frame 0 in the ring is visible to every lane of the group
+  if (e.valid && p.reset_obs_stacked != nullptr) {
+    const double* fr0 = p.hist + static_cast<size_t>(env) * p.history * e.ng * p.obs_dim;
+    write_stacked_row(p, p.reset_obs_stacked, env, 0, gl, G, [&](int i) { return conv ? s.base[prog[i]] : fr0[i]; });
+  }
+}
+
+// MODE_RESET launch: get_state (:213-230): [P_bus | Q_bus | pv | q | vm | va(deg)] restricted to state_space (cold program)
+template <int G>
+__device__ __forceinline__ void write_state(const Params& p, const Hot& h, const Slab& s, const EnvPass& e) {
+  const int env = e.env, gl = e.gl;
+  const bool valid = e.valid;
+  double* o = p.state + static_cast<size_t>(env) * p.state_dim;
+  for (int idx = gl; idx < p.state_dim; idx += G) {
+    const unsigned src = __ldg(p.state_src + idx);
+    const int kind = static_cast<int>(src >> 28), ix = static_cast<int>(src & 0x0FFFFFFFu);
+    double v = 0.0;
+    if (kind == OBS_PBUS) v = s.node(h.node_of_bus[ix])[A_BP].x;
+    else if (kind == OBS_QBUS) v = s.node(h.node_of_bus[ix])[A_BP].y;
+    else if (kind == OBS_PV) v = s.pv[ix];
+    else if (kind == OBS_QSG) v = s.q[ix];
+    else if (kind == OBS_VM) v = s.node(h.node_of_bus[ix])[A_VV].x;
+    else if (kind == OBS_VA_DEG) v = s.node(h.node_of_bus[ix])[A_VV].y * kRad2Deg;
+    if (valid) o[idx] = v;
+  }
+}
+
+// One persistent kernel for every mode: groups of G lanes each solve one env per pass; the CTA walks its envs in rounds.
 // RECORD (MODE_STEP only): the epilogue also writes the env's tester record row (see Params::record) from the values it
 // already holds. HIST (MODE_STEP only, handles with history): the epilogue also writes the env's newest observation frame
 // into its slot of the ring and, when Params::obs_stacked is set, the stacked row. AUTORESET (MODE_STEP only, not with
 // RECORD): after the step, every env that terminated runs the reset of MODE_RESET in the same launch (see the end of the
-// persistent loop). Template flags, so the instantiations without them are the same code as before they existed.
+// persistent loop). Template flags, so the instantiations without them carry none of their code.
 template <int G, int MODE, bool DENSE = false, bool RECORD = false, bool HIST = false, bool AUTORESET = false>
 __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_constant__ Params p) {
   static_assert(!DENSE || G == 32, "the dense fallback uses one warp per env");
@@ -877,11 +1359,14 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
   const int n_helper_threads = (MODE == MODE_STEP) ? p.helper_threads : 0;
   const int n_solver_threads = blockDim.x - n_helper_threads;
   const bool is_helper = (MODE == MODE_STEP) && threadIdx.x >= n_solver_threads;
-  const int hl_bytes = p.hot_layout.bytes;
   const int gl = threadIdx.x % G;
   const int gidx = is_helper ? 0 : threadIdx.x / G;
   const int epb = n_solver_threads / G;
+  const int hl_bytes = p.hot_layout.bytes;
   const int npq = p.npq, n = p.n_bus, nl = p.n_load, ng = p.n_sgen;
+  // scratch: [0, n_sgen) the helper warps' new sgen.p_mw (MODE_STEP) / the previous PV-bus voltages (MODE_DROOP), then the
+  // per-warp partials of the multi-warp group reductions, then - only when they do not fit the node records - the staged
+  // loads (see prologue)
   Slab s;
   {
     double2* base = reinterpret_cast<double2*>(smem_raw + hl.bytes) + static_cast<size_t>(gidx) * p.env_stride2;
@@ -890,129 +1375,35 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
     s.pv = reinterpret_cast<double*>(base + p.pvq_off2);
     s.q = s.pv + ng;
     s.scratch = reinterpret_cast<double*>(base + p.scratch_off2);
+    s.red = s.scratch + ng;
+    s.stage = s.scratch + ng + (G > 32 ? 10 * (G / 32) : 0);
   }
-  // scratch: [0, n_sgen) the helper warps' new sgen.p_mw (MODE_STEP) / the previous PV-bus voltages (MODE_DROOP), then the
-  // per-warp partials of the multi-warp group reductions, then - only when they do not fit there - the staged loads.
-  // Staged (scaled) load p / q of the prologue, 2 n_load doubles: they normally live in the Newton fields of the node
-  // records (UP .. R = 12 contiguous doubles per record), which are dead until the flat start overwrites them.
-  double* next_row = s.scratch;
-  double* red_scratch = s.scratch + ng;
   const bool stage_rec = p.stage_in_records != 0;
-  double* stage_lin = s.scratch + ng + (G > 32 ? 10 * (G / 32) : 0);
   const uint32_t k0 = static_cast<uint32_t>(p.seed), k1 = static_cast<uint32_t>(p.seed >> 32);
 
   // AUTORESET: after the step pass over the envs of a round, a warp (G <= 32) or group (G > 32) with an env that terminated
   // runs a reset pass over the same envs (see below) before it moves to the next round
   bool ended = false;         // MODE_STEP: the group's env terminated in the step pass
   bool reset_next = false;    // the next iteration is the reset pass over the envs of this round
-  // (AUTORESET spelled out in the two expressions below: the other instantiations keep the loop exactly as it was)
   for (int base = blockIdx.x * epb; base < p.nb; base += (AUTORESET && reset_next) ? 0 : gridDim.x * epb) {
     const bool auto_pass = AUTORESET && reset_next;
     reset_next = false;
     if (is_helper) {
-      // ---- helper warps: next profile row of every env of this round (reference _set_demand_and_pv :491-513:
-      //      t = self.steps before the increment) + |N(0,1)| * std noise in Box-Muller pairs (2m, 2m+1) over the
-      //      elements [pv | load_p | load_q]; new pv goes to the env's scratch (for the obs), loads straight to HBM.
-      //      Two dependent global round trips in total: (A) the per-env scalars of the whole round -> shared memory,
-      //      (B) the profile values, four work items per thread in flight, addresses selected without branches. ----
-      const int n_elem = ng + 2 * nl, n_pair = (n_elem + 1) / 2, n_work = epb * n_pair;
-      const int ht = threadIdx.x - n_solver_threads, T = n_helper_threads;
-      int4* hs = reinterpret_cast<int4*>(smem_raw + p.helper_off);     // per env: (row lo, row hi, steps, episode)
-#ifdef MAPDN_HOST_EMU
-      emu::bar_sync(15, T);
-#else
-      asm volatile("bar.sync 15, %0;" ::"r"(T) : "memory");     // helper threads only: the previous round's reads of hs are done
-#endif
-      for (int e = ht; e < epb; e += T) {
-        const int env_h = base + e;
-        int4 v = make_int4(0, 0, 0, 0);
-        if (env_h < p.nb) {
-          const int steps_h = p.steps[env_h];
-          long long nrow = p.start_row[env_h] + steps_h;
-          if (nrow > p.n_rows - 1) nrow = p.n_rows - 1;
-          v = make_int4(static_cast<int>(nrow & 0xFFFFFFFFll), static_cast<int>(nrow >> 32), steps_h,
-                        static_cast<int>(p.episode[env_h]));
-        }
-        hs[e] = v;
-      }
-#ifdef MAPDN_HOST_EMU
-      emu::bar_sync(15, T);
-#else
-      asm volatile("bar.sync 15, %0;" ::"r"(T) : "memory");     // helper threads only
-#endif
-      named_bar_sync(1, blockDim.x);                   // the solvers have read the current rows
-      constexpr int U = 4;
-      for (int w0 = ht; w0 < n_work; w0 += U * T) {
-        double val[U][2], sd[U][2];
-        int e_[U], m_[U];
-        bool ok[U];
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-          const int w = w0 + u * T;
-          ok[u] = w < n_work;
-          const int e = ok[u] ? w / n_pair : 0;
-          e_[u] = e; m_[u] = w - e * n_pair;
-          ok[u] = ok[u] && (base + e < p.nb);
-          const int4 sc = hs[e];
-          const long long nrow = (static_cast<long long>(sc.y) << 32) | static_cast<unsigned>(sc.x);
-#pragma unroll
-          for (int k = 0; k < 2; ++k) {
-            const int el = min(2 * m_[u] + k, n_elem - 1);          // an odd n_elem re-reads the last element (not stored)
-            const bool is_pv = el < ng, is_lp = el < ng + nl;
-            const int j = is_pv ? el : (is_lp ? el - ng : el - ng - nl);
-            const double* src = is_pv ? p.prof_pv + nrow * ng : (is_lp ? p.prof_lp + nrow * nl : p.prof_lq + nrow * nl);
-            const double* sds = is_pv ? p.pv_std : (is_lp ? p.lp_std : p.lq_std);
-            val[u][k] = ok[u] ? __ldg(src + j) : 0.0;
-            sd[u][k] = ok[u] ? __ldg(sds + j) : 0.0;
-          }
-        }
-        // one copy of Philox + log + sqrt + sincos (not four: the solver warps need the instruction cache); the work
-        // item is picked out of the registers with select chains
-#pragma unroll 1
-        for (int u = 0; u < U; ++u) {
-          bool oku = ok[0]; int e = e_[0], m = m_[0];
-          double va = val[0][0], vb = val[0][1], sa = sd[0][0], sb = sd[0][1];
-#pragma unroll
-          for (int q = 1; q < U; ++q)
-            if (u == q) { oku = ok[q]; e = e_[q]; m = m_[q]; va = val[q][0]; vb = val[q][1]; sa = sd[q][0]; sb = sd[q][1]; }
-          if (!oku) continue;
-          const int env_h = base + e;
-          const int4 sc = hs[e];
-          RngKey key_h{k0, k1, static_cast<uint32_t>(p.env_id_offset + env_h), static_cast<uint32_t>(sc.w) * 8u};
-          double z0 = 0.0, z1 = 0.0;
-          if (p.add_noise) half_normal_pair(key_h, static_cast<uint32_t>(sc.z), m, z0, z1);
-          double* pv_next = reinterpret_cast<double*>(reinterpret_cast<double2*>(smem_raw + hl_bytes) +
-                                                       static_cast<size_t>(e) * p.env_stride2 + p.scratch_off2);
-          const size_t hL = static_cast<size_t>(env_h) * nl, hG = static_cast<size_t>(env_h) * ng;
-#pragma unroll
-          for (int k = 0; k < 2; ++k) {
-            const int el = 2 * m + k;
-            if (el >= n_elem) break;
-            const double v = (k == 0) ? va + sa * z0 : vb + sb * z1;
-            const bool is_pv = el < ng, is_lp = el < ng + nl;
-            double* dst = is_pv ? p.cur_pv + hG + el : (is_lp ? p.cur_pl + hL + (el - ng) : p.cur_ql + hL + (el - ng - nl));
-            *dst = v;
-            if (is_pv) pv_next[el] = v;
-          }
-        }
-      }
-      named_bar_arrive(2, blockDim.x);                 // new pv of every env is in shared memory
+      helper_draw_rows(p, smem_raw, base, epb, n_solver_threads, n_helper_threads, k0, k1, ng, nl, hl_bytes);
       continue;
     }
     // The pass runs in mode M: the kernel's own MODE, or MODE_RESET in the auto-reset pass, so that a launched reset and an
     // auto-reset run the same code. The auto-reset pass differs from a reset launch only where the step launch's
     // parameters say otherwise: the selection is `ended`, the start is sampled and noise is on (reference reset() :118),
     // the observation goes to Params::reset_obs, and frame 0 of the new episode to the ring and Params::reset_obs_stacked.
-    // (One loop body for both passes, not a function instantiated per mode: the instantiations without AUTORESET keep their
-    // code as it was.)
     const int M = auto_pass ? static_cast<int>(MODE_RESET) : MODE;
     int env = base + gidx;
     bool valid = env < p.nb;
     if (!valid) env = p.nb - 1;
     if (auto_pass) { if (!ended) valid = false; }
     else if (M == MODE_RESET && p.mask != nullptr && !p.mask[env]) valid = false;
-    const size_t eL = static_cast<size_t>(env) * nl, eG = static_cast<size_t>(env) * ng,
-                 eN = static_cast<size_t>(env) * n;
+    const EnvPass e{M, auto_pass, env, valid, static_cast<size_t>(env) * nl, static_cast<size_t>(env) * ng,
+                    static_cast<size_t>(env) * n, gidx, gl, npq, n, nl, ng};
 
     RngKey key{k0, k1, static_cast<uint32_t>(p.env_id_offset + env), 0u};
     long long start = 0;
@@ -1032,97 +1423,10 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
     bool solved = false;
     bool dr_active = valid;      // MODE_DROOP: this env has not met the stopping rule yet
     int dr_iters = 0;
-    double* v_last = s.scratch;                    // MODE_DROOP: PV-bus voltages of the previous power flow [n_sgen]
     const int n_rounds = (M == MODE_RESET) ? kMaxResetAttempts : (M == MODE_DROOP ? p.droop_max_ite : 1);
     for (int round = 0; round < n_rounds; ++round) {
-      // ---------------- prologue: element values -> sgen p/q and bus injections ----------------
-      if (M == MODE_RESET) {
-        int day, hour, interval;
-        if (!auto_pass && p.start_dhi != nullptr) {                 // manual_reset :137-152
-          day = p.start_dhi[env * 3 + 0]; hour = p.start_dhi[env * 3 + 1]; interval = p.start_dhi[env * 3 + 2];
-        } else {                                                    // :111-113, :381-398
-          const u32x4 r = philox4x32_10(0u, static_cast<uint32_t>(attempt), key.env, key.c3base + kStreamTime, k0, k1);
-          hour = static_cast<int>(__umulhi(r.x, 24u));
-          day = static_cast<int>(__umulhi(r.y, static_cast<uint32_t>(p.n_day_choices)));
-          interval = static_cast<int>(__umulhi(r.z, static_cast<uint32_t>(p.steps_per_hour)));
-        }
-        start = interval + static_cast<long long>(hour) * p.steps_per_hour +
-                static_cast<long long>(day) * 24 * p.steps_per_hour;          // :445
-        // a manual start outside the store is clamped to the last window that fits (the host shims validate and
-        // raise; the kernel only guarantees in-bounds reads)
-        start = max(0ll, min(start, p.n_rows - 1 - p.episode_limit));
-      }
-      long long row = 0;
-      if (M == MODE_RESET) { row = start + 1; if (row > p.n_rows - 1) row = p.n_rows - 1; }   // t = steps = 1
-      const uint32_t c1 = kResetFlag | static_cast<uint32_t>(attempt);
-      // (1) coalesced, independent loads of the env's element values into shared memory
-      if (M != MODE_DROOP || round == 0) {          // droop: later rounds only change q (in shared memory)
-#pragma unroll 4
-      for (int j = gl; j < ng; j += G) {
-        double pv, q;
-        if (M == MODE_SOLVE || M == MODE_DROOP) {
-          pv = p.in_pv[eG + j]; q = (M == MODE_SOLVE) ? p.in_q[eG + j] : 0.0;     // droop starts from q = 0 (:107)
-          if (M == MODE_DROOP) v_last[j] = 100.0;                                    // :123
-        } else if (M == MODE_STEP) {
-          pv = p.cur_pv[eG + j];
-          q = clip_q(p.actions[eG + j], pv, __ldg(p.s_max + j));             // :553
-        } else {
-          pv = __ldg(p.prof_pv + row * ng + j);
-          if (auto_pass || p.add_noise) pv += __ldg(p.pv_std + j) * half_normal(key, c1, j);   // :498
-          q = 0.0;
-          if (p.reset_action) {                                               // :120-122, :334-338
-            const u32x4 r = philox4x32_10(j, static_cast<uint32_t>(attempt), key.env, key.c3base + kStreamAction, k0, k1);
-            const double a = p.action_low + (p.action_high - p.action_low) * u53(r.x, r.y);
-            q = clip_q(a, pv, __ldg(p.s_max + j));
-          }
-          if (valid) p.cur_pv[eG + j] = pv;
-        }
-        s.pv[j] = pv; s.q[j] = q;
-      }
-      }
-      // (droop re-stages the loads every round: the staging area is overwritten by the Newton iteration)
-      // Written once, instantiated for the two staging places (block-uniform choice): a branch per access inside the
-      // loops would cost time in every step.
-      auto stage_and_gather = [&](auto stg) {
-#pragma unroll 4
-        for (int l = gl; l < nl; l += G) {
-          double pl, ql;
-          if (M == MODE_SOLVE || M == MODE_DROOP) { pl = p.in_pl[eL + l]; ql = p.in_ql[eL + l]; }
-          else if (M == MODE_STEP) { pl = p.cur_pl[eL + l]; ql = p.cur_ql[eL + l]; }
-          else {
-            pl = __ldg(p.prof_lp + row * nl + l);
-            ql = __ldg(p.prof_lq + row * nl + l);
-            if (auto_pass || p.add_noise) {                                      // :503, :508
-              pl += __ldg(p.lp_std + l) * half_normal(key, c1, ng + l);
-              ql += __ldg(p.lq_std + l) * half_normal(key, c1, ng + nl + l);
-            }
-            if (valid) { p.cur_pl[eL + l] = pl; p.cur_ql[eL + l] = ql; }
-          }
-          const double sc = __ldg(p.lscale + l);
-          *stg(l) = pl * sc; *stg(nl + l) = ql * sc;
-        }
-        if (!hot_ready) { stage_hot_wait(&stage_bar); hot_ready = true; }
-        grp_sync<G>(gidx);
-        // (2) A.1: PD/QD per bus, Sbus = -(PD + jQD)/baseMVA
-        for (int i = gl; i < npq; i += G) {
-          double pd = 0.0, qd = 0.0;
-#pragma unroll 1
-          for (int t = h.lptr[i], te = h.lptr[i + 1]; t < te; ++t) { const int l = h.lidx[t]; pd += *stg(l); qd += *stg(nl + l); }
-#pragma unroll 1
-          for (int t = h.sptr[i], te = h.sptr[i + 1]; t < te; ++t) {
-            const int g = h.sidx[t];
-            const double sc = __ldg(p.sscale + g);
-            pd -= s.pv[g] * sc; qd -= s.q[g] * sc;
-          }
-          s.node(i)[A_SP] = make_double2(-pd * p.inv_base, -qd * p.inv_base);
-        }
-      };
-      if (stage_rec) stage_and_gather([&](int k) -> double* { return s.base + (k / 12) * (2 * kNodeArrays2) + 2 * A_UP + (k % 12); });
-      else stage_and_gather([&](int k) -> double* { return stage_lin + k; });
-      grp_sync<G>(gidx);
-      if (M == MODE_STEP) named_bar_arrive(1, blockDim.x);   // the current rows are consumed: the helper may overwrite them
-
-      // ---------------- Newton-Raphson ----------------
+      if (M == MODE_RESET) start = reset_start(p, e, key, attempt);
+      prologue<G>(p, h, s, e, key, start, attempt, round, stage_rec, hot_ready, &stage_bar);
       PROF(1)
       if (DENSE) {
         double* ws = p.dense_ws + (static_cast<size_t>(blockIdx.x) * epb + gidx) * p.dense_stride;
@@ -1139,14 +1443,16 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
         // relaxed fixed-point loop of pf_droop_matpower_all.m:121-152: stop when ||v_pv - v_pv_last||_2 < tol, else
         // q <- (1 - gain) q + gain q_droop(v). An env that has stopped keeps its q, so the power flows it still runs
         // alongside the others of its warp reproduce its final state; the last allowed round does not move q either
-        // (the script reports the q of the last power flow).
+        // (the script reports the q of the last power flow). (Inline: as a function it changes the droop kernels'
+        // register allocation.)
+        double* v_last = s.scratch;
         double part[1] = {0.0};
         const bool no_max[1] = {false};
         for (int j = gl; j < ng; j += G) {
           const double dv = v_last[j] - s.node(__ldg(p.sgen_node + j))[A_VV].x;
           part[0] += dv * dv;
         }
-        grp_reduce<G, 1>(gidx, gl, part, no_max, red_scratch);
+        grp_reduce<G, 1>(gidx, gl, part, no_max, s.red);
         const bool stop = sqrt(part[0]) < p.droop_tol;
         if (dr_active) { dr_iters = round + 1; if (stop) dr_active = false; }
         if (grp_exit<G>(!dr_active) || round == n_rounds - 1) break;
@@ -1168,179 +1474,37 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
       grp_sync<G>(gidx);
     }
 
-    // ---------------- epilogue ----------------
-    // divergence branch (reference :188-196): fall back to the previous solution kept in HBM
-    if (M == MODE_STEP && !conv) {
-      for (int i = gl; i < npq; i += G) {
-        const int b = __ldg(p.bus_of_node + i);
-        const double vm = p.res_vm[eN + b], va = p.res_va[eN + b];
-        double sn, cs;
-        sincos(va, &sn, &cs);
-        double2* nd = s.node(i);
-        nd[A_VV] = make_double2(vm, va);
-        nd[A_EF] = make_double2(vm * cs, vm * sn);
-        nd[A_SP] = make_double2(-p.res_p[eN + b] * p.inv_base, -p.res_q[eN + b] * p.inv_base);
-      }
-    }
-    grp_sync<G>(gidx);
-    // a reset whose kMaxResetAttempts draws all diverged keeps the env's previous state and reports it (reset_ok)
+    fallback_and_slack<G>(p, s, e, conv, iters);
+    PROF(7)
     const bool kExplicit = (M == MODE_SOLVE || M == MODE_DROOP);     // explicit inputs / outputs, no env state
     const bool write_res = valid && (kExplicit || conv);
-    if (M == MODE_RESET && valid && gl == 0 && p.reset_ok != nullptr) p.reset_ok[env] = conv ? 1 : 0;
-    if (!kExplicit && valid && gl == 0) p.nr_iters[env] = conv ? iters : p.max_iter;
-
-    // slack injection (pfsoln, SURVEY A.5): S0 = V0 conj(Ybus[0,:] V) -> sentinel record's SP
-    {
-      const double vv = p.vm0 * p.vm0;
-      double P0 = p.ysl_g0 * vv, Q0 = -p.ysl_b0 * vv;
-      for (int k = 0; k < p.n_slack_adj; ++k) {
-        const int i = __ldg(p.sl_node + k);
-        const double g = __ldg(p.sl_y + 2 * k), b = __ldg(p.sl_y + 2 * k + 1);
-        const double2 vi = s.node(i)[A_EF];
-        const double cc = p.e0 * vi.x + p.f0 * vi.y, ss = p.f0 * vi.x - p.e0 * vi.y;   // V0 Vi cos/sin(t0 - ti)
-        P0 += g * cc + b * ss;
-        Q0 += g * ss - b * cc;
-      }
-      if (gl == 0) s.node(npq)[A_SP] = make_double2(P0, Q0);
-    }
-    PROF(7)
-    // sgen.q_mvar after the step: the clipped action, or the previous q on divergence (:189-196)
-    double sum_q_eff = 0.0, sum_q_try = 0.0;
-    if (M == MODE_STEP) {
-      for (int j = gl; j < ng; j += G) {
-        const double q_try = s.q[j];
-        const double q_eff = conv ? q_try : p.cur_q[eG + j];
-        sum_q_try += fabs(q_try);
-        sum_q_eff += fabs(q_eff * __ldg(p.sscale + j));     // res_sgen.q_mvar = q * scaling (:604-605)
-        s.q[j] = q_eff;
-        if (write_res) p.cur_q[eG + j] = q_eff;
-      }
-    }
-    // the helper warp has drawn the next profile row meanwhile: take over the new sgen.p_mw (Appendix B.3: the
-    // observation mixes this solve's bus results with the NEXT row's PV)
-    // record row [pv | q | P_bus | Q_bus | vm | line loss] (the order of the reference tester's getters): exactly what
-    // mapdn_get_field returns after this step. pv is already the next profile row (reference :199 runs before the
-    // tester's getters); q is the effective one; a diverged env reports its previous results, read back from HBM.
     [[maybe_unused]] double* const rec = RECORD ? p.record + static_cast<size_t>(env) * p.record_stride : nullptr;
-    if (M == MODE_STEP) {
-      named_bar_sync(2, blockDim.x);
-      for (int j = gl; j < ng; j += G) s.pv[j] = next_row[j];
-      if constexpr (RECORD) {
-        if (valid)
-          for (int j = gl; j < ng; j += G) { rec[j] = s.pv[j]; rec[ng + j] = s.q[j]; }
-      }
-    }
-    grp_sync<G>(gidx);
+    StepStats st;
+    effective_q_and_next_row<G, RECORD>(p, s, e, conv, write_res, rec, st);
     PROF(8)
-    // res_bus columns per node (BP) and the "demand" columns of get_obs (OP = BP + sgens of the bus's own zone)
-    for (int i = gl; i <= npq; i += G) {
-      double2* nd = s.node(i);
-      const double2 sp = nd[A_SP];
-      double2 bp = make_double2(-sp.x * p.base_mva, -sp.y * p.base_mva);
-      if (p.has_shunt) {                   // warp-uniform; pandapower adds the bus shunts' p/q (x vm^2) to res_bus
-        const double2 ef = nd[A_EF];
-        const double v2 = ef.x * ef.x + ef.y * ef.y;
-        bp.x += __ldg(p.sh_g + i) * v2; bp.y -= __ldg(p.sh_b + i) * v2;
-      }
-      double2 op = bp;
-#pragma unroll 1
-      for (int t = h.xptr[i], te = h.xptr[i + 1]; t < te; ++t) { const int g = h.xidx[t]; op.x += s.pv[g]; op.y += s.q[g]; }
-      nd[A_BP] = bp; nd[A_OP] = op;
-    }
-    grp_sync<G>(gidx);
-    // per-bus results + voltage statistics (reference _calc_reward :584-596, :610)
-    double cnt_lo = 0, cnt_hi = 0, sum_dev = 0, sum_v = 0, max_drop = 0, max_rise = 0, sum_bar = 0;
-    const double v_ref = 0.5 * (p.v_lower + p.v_upper);
-#pragma unroll 4
-    for (int b = gl; b < n; b += G) {
-      const double2* nd = s.node(h.node_of_bus[b]);
-      const double2 vv = nd[A_VV], bp = nd[A_BP];
-      const double v = vv.x, th = vv.y;
-      if (kExplicit) {
-        if (valid) {
-          if (p.out_vm) p.out_vm[eN + b] = v;
-          if (p.out_va) p.out_va[eN + b] = th * kRad2Deg;
-          if (p.out_p) p.out_p[eN + b] = bp.x;
-          if (p.out_q) p.out_q[eN + b] = bp.y;
-        }
-      } else {
-        if (write_res) {
-          p.res_vm[eN + b] = v; p.res_va[eN + b] = th; p.res_p[eN + b] = bp.x; p.res_q[eN + b] = bp.y;
-        }
-        if constexpr (RECORD) {         // consecutive lanes, consecutive buses: coalesced like the res_* stores
-          if (valid) {
-            rec[2 * ng + b] = conv ? bp.x : p.res_p[eN + b];
-            rec[2 * ng + n + b] = conv ? bp.y : p.res_q[eN + b];
-            rec[2 * ng + 2 * n + b] = v;                    // on divergence: reloaded from res_vm above
-          }
-        }
-        if (M == MODE_STEP) {
-          cnt_lo += (v < p.v_lower) ? 1.0 : 0.0;
-          cnt_hi += (v > p.v_upper) ? 1.0 : 0.0;
-          sum_dev += fabs(v - v_ref);
-          sum_v += v;
-          max_drop = fmax(max_drop, (v < p.v_lower) ? (p.v_lower - v) : 0.0);
-          max_rise = fmax(max_rise, (v > p.v_upper) ? (v - p.v_upper) : 0.0);
-          sum_bar += barrier_fn(p.barrier, v);
-        }
-      }
-    }
-    // line losses: res_line.pl_mw = Re(Sf + St) (SURVEY A.5), 4 static coefficients per line. The two tables are either
-    // part of the staged blob (LDS) or cold in global memory (read-only path): one block-uniform branch, two typed loops.
-    double sum_pl = 0.0;
-    {
-      const size_t ePL = static_cast<size_t>(env) * p.n_line;
-      auto lines = [&](const ushort2* __restrict__ ln, const double2* __restrict__ lc) {
-#pragma unroll 4
-        for (int k = gl; k < p.n_line; k += G) {
-          const ushort2 ft = ln[k];
-          const double2 vf = s.node(ft.x)[A_EF], vt = s.node(ft.y)[A_EF];
-          const double cc = vf.x * vt.x + vf.y * vt.y, ss = vf.y * vt.x - vf.x * vt.y;
-          const double2 c01 = lc[2 * k], c23 = lc[2 * k + 1];
-          const double pl = c01.x * (vf.x * vf.x + vf.y * vf.y) + c01.y * (vt.x * vt.x + vt.y * vt.y) + c23.x * cc + c23.y * ss;
-          sum_pl += pl;
-          if (kExplicit) { if (valid && p.out_pl) p.out_pl[ePL + k] = pl; }
-          else if (write_res) p.res_pl[ePL + k] = pl;
-          if constexpr (RECORD) {
-            if (valid) rec[2 * ng + 3 * n + k] = conv ? pl : p.res_pl[ePL + k];
-          }
-        }
-      };
-      if (h.in_blob) lines(reinterpret_cast<const ushort2*>(smem_raw + hl.line_nodes), reinterpret_cast<const double2*>(smem_raw + hl.line_c));
-      else lines(reinterpret_cast<const ushort2*>(p.line_nodes), reinterpret_cast<const double2*>(p.line_c));
-    }
+    bus_results<G, RECORD>(p, h, s, e, conv, write_res, rec, st);
     PROF(9)
     if (kExplicit) {
-      if (M == MODE_DROOP) {
-        double tot[1] = {sum_pl};
-        const bool no_max[1] = {false};
-        grp_reduce<G, 1>(gidx, gl, tot, no_max, red_scratch);
-        if (valid) {
-          for (int j = gl; j < ng; j += G) p.droop_q_out[eG + j] = s.q[j];
-          if (gl == 0) { p.droop_loss_out[env] = tot[0]; p.out_iters[env] = dr_iters; }
-        }
-      }
-      if (valid && gl == 0) {
-        if (M == MODE_SOLVE && p.out_iters) p.out_iters[env] = conv ? iters : p.max_iter;
-        if (p.out_conv) p.out_conv[env] = conv ? 1 : 0;
-      }
-      grp_sync<G>(gidx);
+      explicit_outputs<G>(p, s, e, conv, iters, dr_iters, st.sum_pl);
       continue;
     }
-
+    // (the reward and the observation gather stay inline: as functions they change the register allocation of the
+    // auto-reset instantiations)
     if (M == MODE_STEP) {
+      // reward (reference _calc_reward :612-618, :192), the 11 info scalars and the step counters
       {
-        double rv[10] = {cnt_lo, cnt_hi, sum_dev, sum_v, sum_bar, max_drop, max_rise, sum_pl, sum_q_eff, sum_q_try};
+        double rv[10] = {st.cnt_lo, st.cnt_hi, st.sum_dev, st.sum_v, st.sum_bar, st.max_drop, st.max_rise, st.sum_pl,
+                         st.sum_q_eff, st.sum_q_try};
         const bool rmax[10] = {false, false, false, false, false, true, true, false, false, false};
-        grp_reduce<G, 10>(gidx, gl, rv, rmax, red_scratch);
-        cnt_lo = rv[0]; cnt_hi = rv[1]; sum_dev = rv[2]; sum_v = rv[3]; sum_bar = rv[4];
-        max_drop = rv[5]; max_rise = rv[6]; sum_pl = rv[7]; sum_q_eff = rv[8]; sum_q_try = rv[9];
+        grp_reduce<G, 10>(gidx, gl, rv, rmax, s.red);
+        st.cnt_lo = rv[0]; st.cnt_hi = rv[1]; st.sum_dev = rv[2]; st.sum_v = rv[3]; st.sum_bar = rv[4];
+        st.max_drop = rv[5]; st.max_rise = rv[6]; st.sum_pl = rv[7]; st.sum_q_eff = rv[8]; st.sum_q_try = rv[9];
       }
       const double inv_n = 1.0 / n;
-      const double pct = (cnt_lo + cnt_hi) * inv_n;
-      const double q_loss = sum_q_eff / ng;
-      const double v_loss = sum_bar * inv_n * p.voltage_weight;
-      const double loss = p.use_line_weight ? (sum_pl / p.n_line) * p.line_weight + v_loss
+      const double pct = (st.cnt_lo + st.cnt_hi) * inv_n;
+      const double q_loss = st.sum_q_eff / ng;
+      const double v_loss = st.sum_bar * inv_n * p.voltage_weight;
+      const double loss = p.use_line_weight ? (st.sum_pl / p.n_line) * p.line_weight + v_loss
                                             : q_loss * p.q_weight + v_loss;     // :612-618
       double reward = -loss;
       if (!conv) reward -= 200.0;                                               // :192
@@ -1357,31 +1521,26 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
         // instructions per env instead of eleven from lane 0 - it matters when `info` is pinned host memory
         double* o = p.info + static_cast<size_t>(env) * 11;
         const double i3 = (!conv || pct > 1e-3) ? 0.0 : 1.0;                     // :589, :195
-        const double i9 = conv ? q_loss : sum_q_try / ng, i10 = conv ? 0.0 : 1.0;
+        const double i9 = conv ? q_loss : st.sum_q_try / ng, i10 = conv ? 0.0 : 1.0;
         for (int k = gl; k < 11; k += G) {
           double v = pct;                                                         // select chain, no divergent branches
-          v = (k == 1) ? cnt_lo * inv_n : v; v = (k == 2) ? cnt_hi * inv_n : v; v = (k == 3) ? i3 : v;
-          v = (k == 4) ? sum_dev * inv_n : v; v = (k == 5) ? sum_v * inv_n : v; v = (k == 6) ? max_drop : v;
-          v = (k == 7) ? max_rise : v; v = (k == 8) ? sum_pl : v; v = (k == 9) ? i9 : v; v = (k == 10) ? i10 : v;
+          v = (k == 1) ? st.cnt_lo * inv_n : v; v = (k == 2) ? st.cnt_hi * inv_n : v; v = (k == 3) ? i3 : v;
+          v = (k == 4) ? st.sum_dev * inv_n : v; v = (k == 5) ? st.sum_v * inv_n : v; v = (k == 6) ? st.max_drop : v;
+          v = (k == 7) ? st.max_rise : v; v = (k == 8) ? st.sum_pl : v; v = (k == 9) ? i9 : v; v = (k == 10) ? i10 : v;
           o[k] = v;
         }
       }
-    } else {  // MODE_RESET
-      for (int j = gl; j < ng; j += G) if (valid) p.cur_q[eG + j] = s.q[j];
-      if (valid && gl == 0) {
-        p.steps[env] = 1;                         // :100
-        p.sum_rewards[env] = 0.0;                 // :101
-        p.start_row[env] = start;
-        p.episode[env] = p.episode[env] + 1u;
-      }
+    } else {
+      reset_bookkeeping<G>(p, s, e, start);
     }
     PROF(10)
-    // observations of the new state (reference get_obs :232-316): a pure gather - the program maps every entry to a
-    // double inside this env's slab, or to a constant-zero slot for the padding. A lane copies 16 bytes per
-    // instruction (two fp64 / four fp32 entries) and consecutive lanes consecutive 16-byte pieces, so one store
-    // instruction writes 128 contiguous bytes per env (full lines when the destination is pinned host memory).
-    // obs_skip_off: entries reading that slot (the padding) are not stored.
-    // (the destination is spelled out at each use: a local copy of p.obs would change the code of the other instantiations)
+    // Observations of the new state (reference get_obs :232-316): a pure gather - the program maps every entry to a double
+    // inside this env's slab, or to a constant-zero slot for the padding. A lane copies 16 bytes per instruction (two fp64 /
+    // four fp32 entries) and consecutive lanes consecutive 16-byte pieces, so one store instruction writes 128 contiguous bytes
+    // per env (full lines when the destination is pinned host memory). obs_skip_off: entries reading that slot (the padding)
+    // are not stored. The auto-reset pass writes to Params::reset_obs.
+    // (the destination is spelled out at each use: a local copy of p.obs changes the register allocation of the
+    // instantiations without auto-reset)
     if (((auto_pass ? p.reset_obs : p.obs) != nullptr || (M == MODE_STEP && p.obs32 != nullptr)) && valid) {
       const bool compact = p.obs_compact_len > 0;          // rows without the per-agent padding (staged host path)
       const int tot = compact ? p.obs_compact_len : ng * p.obs_dim;
@@ -1437,58 +1596,9 @@ __global__ void __launch_bounds__(G > 32 ? 640 : 384) env_kernel(const __grid_co
       if (h.in_blob && !compact) gather(reinterpret_cast<const uint16_t*>(smem_raw + hl.obs_off), std::false_type{});
       else gather(compact ? p.obs_compact_prog : p.obs_off, std::true_type{});
     }
-    if (HIST && AUTORESET && auto_pass) {
-      // frame 0 of the new episode, what reset_frame_kernel writes after a reset launch: the slab through the padded
-      // program when the reset converged (the state in HBM holds the same values), else the state in HBM (a reset whose
-      // draws all diverged keeps the old res_*, which its slab does not hold; the group's stores above must be visible to
-      // every lane of the group first). Its stacked row (write_stacked_row at f = 0): H - 1 zero frames, then frame 0.
-      grp_sync<G>(gidx);
-      if (valid) {
-        const int od = p.obs_dim, tot = ng * od, blk = p.history * od;
-        const uint16_t* prog = h.in_blob ? reinterpret_cast<const uint16_t*>(smem_raw + hl.obs_off) : p.obs_off;
-        auto frame0 = [&](int i) { return conv ? s.base[prog[i]] : obs_entry(p, env, i); };
-        double* fr = p.hist + static_cast<size_t>(env) * p.history * tot;
-        for (int i = gl; i < tot; i += G) fr[i] = frame0(i);
-        if (p.reset_obs_stacked != nullptr) {
-          double* o = p.reset_obs_stacked + static_cast<size_t>(env) * ng * blk;
-          for (int e = gl; e < ng * blk; e += G) {
-            const int a = e / blk, r = e - a * blk;
-            o[e] = r < blk - od ? 0.0 : frame0(a * od + r - (blk - od));
-          }
-        }
-      }
-    } else if constexpr (HIST) {
-      // frame f = steps - 1 of this step into its ring slot, through the padded program whatever layout (compact, fp32,
-      // none) the caller's observations take; then the stacked row, whose newest frame comes straight from the slab
-      if (valid) {
-        const int f = steps_old, tot = ng * p.obs_dim;
-        const uint16_t* prog = h.in_blob ? reinterpret_cast<const uint16_t*>(smem_raw + hl.obs_off) : p.obs_off;
-        double* fr = p.hist + (static_cast<size_t>(env) * p.history + f % p.history) * tot;
-        if ((tot & 1) == 0) {
-          for (int c = gl; c < tot / 2; c += G)
-            *reinterpret_cast<double2*>(fr + 2 * c) = make_double2(s.base[prog[2 * c]], s.base[prog[2 * c + 1]]);
-        } else {
-          for (int i = gl; i < tot; i += G) fr[i] = s.base[prog[i]];
-        }
-        if (p.obs_stacked != nullptr) write_stacked_row(p, env, f, gl, G, [&](int i) { return s.base[prog[i]]; });
-      }
-    }
-    if (M == MODE_RESET && !auto_pass && p.state != nullptr) {
-      // get_state (:213-230): [P_bus | Q_bus | pv | q | vm | va(deg)] restricted to state_space (cold program)
-      double* o = p.state + static_cast<size_t>(env) * p.state_dim;
-      for (int idx = gl; idx < p.state_dim; idx += G) {
-        const unsigned src = __ldg(p.state_src + idx);
-        const int kind = static_cast<int>(src >> 28), ix = static_cast<int>(src & 0x0FFFFFFFu);
-        double v = 0.0;
-        if (kind == OBS_PBUS) v = s.node(h.node_of_bus[ix])[A_BP].x;
-        else if (kind == OBS_QBUS) v = s.node(h.node_of_bus[ix])[A_BP].y;
-        else if (kind == OBS_PV) v = s.pv[ix];
-        else if (kind == OBS_QSG) v = s.q[ix];
-        else if (kind == OBS_VM) v = s.node(h.node_of_bus[ix])[A_VV].x;
-        else if (kind == OBS_VA_DEG) v = s.node(h.node_of_bus[ix])[A_VV].y * kRad2Deg;
-        if (valid) o[idx] = v;
-      }
-    }
+    if (HIST && AUTORESET && auto_pass) reset_history<G>(p, h, s, e, conv);
+    else if constexpr (HIST) step_history<G>(p, h, s, e, steps_old);
+    if (M == MODE_RESET && !auto_pass && p.state != nullptr) write_state<G>(p, h, s, e);
     grp_sync<G>(gidx);
     PROF(11)
     if constexpr (AUTORESET) if (!auto_pass) {

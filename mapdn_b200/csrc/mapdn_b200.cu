@@ -135,7 +135,8 @@ __global__ void reset_frame_kernel(const __grid_constant__ Params p) {
   if (gid >= static_cast<long long>(p.nb) * tot) return;
   const int env = static_cast<int>(gid / tot), idx = static_cast<int>(gid - static_cast<long long>(env) * tot);
   if (p.mask != nullptr && !p.mask[env]) return;
-  p.hist[static_cast<size_t>(env) * p.history * tot + idx] = obs_entry(p, env, idx);
+  // one thread per entry: lane idx of tot lanes, so write_frame0's loop runs once
+  write_frame0(p, env, idx, tot, [&](int i) { return obs_entry(p, env, i); });
 }
 
 // mapdn_get_obs_stacked: the stacked rows from the ring and the step counters - the rule the step kernel applies in its
@@ -148,7 +149,7 @@ __global__ void obs_stacked_kernel(const __grid_constant__ Params p) {
   const int env = static_cast<int>(gid / row), c = static_cast<int>(gid - static_cast<long long>(env) * row);
   const double* ring = p.hist + static_cast<size_t>(env) * p.history * p.n_sgen * p.obs_dim;
   // the newest frame is in the ring too: write_stacked_row reads it there, restricted to this thread's piece
-  write_stacked_row(p, env, p.steps[env] - 1, c, row, [&](int i) {
+  write_stacked_row(p, p.obs_stacked, env, p.steps[env] - 1, c, row, [&](int i) {
     return ring[static_cast<size_t>((p.steps[env] - 1) % p.history) * p.n_sgen * p.obs_dim + i];
   });
 }

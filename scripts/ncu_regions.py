@@ -5,10 +5,14 @@ src = open(os.path.join(ROOT, "mapdn_b200/csrc/env_kernel.cuh")).read().splitlin
 marks = [("helpers(reduce,rcp,barrier,stage)", 1), ("nr:init", None, "flat start (pandapower"), ("nr:edges", None, "per-edge terms of"),
          ("nr:F/diag", None, "mismatch F ="), ("nr:elim", None, "forward elimination"), ("nr:backsub", None, "back substitution by"),
          ("nr:update", None, "update (theta"), ("kernel setup", None, "sgen.q_mvar from an action"),
-         ("prologue", None, "prologue: element"), ("nr call/retry", None, "Newton-Raphson ------"),
-         ("epi:reload+slack+q", None, "---------------- epilogue"), ("epi:nextrow", None, "next profile row (reference"),
-         ("epi:BP/OP", None, "res_bus columns per node"), ("epi:bus stats", None, "per-bus results"),
-         ("epi:lines", None, "line losses"), ("epi:reward/info", None, "if (MODE == MODE_STEP) {\n      cnt_lo"), ("epi:obs", None, "observations of the new")]
+         ("helper warps", None, "void helper_draw_rows("), ("reset start", None, "long long reset_start("),
+         ("prologue", None, "void prologue("), ("droop", None, "relaxed fixed-point loop of pf_droop"),
+         ("epi:fallback+slack", None, "void fallback_and_slack("), ("epi:q+nextrow", None, "void effective_q_and_next_row("),
+         ("epi:bus results", None, "void bus_results("), ("epi:lines", None, "line losses: res_line"),
+         ("epi:explicit", None, "void explicit_outputs("), ("epi:reward/info", None, "reward (reference _calc_reward :612-618"),
+         ("epi:reset", None, "void reset_bookkeeping("), ("epi:obs, then history / state calls, ballot", None, "Observations of the new state"),
+         ("epi:history", None, "void step_history("), ("epi:state", None, "void write_state("),
+         ("kernel: setup, prefetch, round loop, nr call", None, "env_kernel(const __grid_constant__")]
 starts = []
 for m in marks:
     if m[1] is not None: starts.append((m[1], m[0])); continue
