@@ -298,6 +298,37 @@ mapdn_status mapdn_step_autoreset(mapdn_env* env, const double* actions_dev /*[B
                                   double* reset_obs_stacked_dev /*or NULL*/, uint8_t* reset_ok_dev /*or NULL*/,
                                   void* stream);
 
+/*
+ * Env state snapshots: save the state of any envs of the batch into device memory and put it back, into the same or
+ * other slots, of this handle or of another one with the same layout.
+ * A snapshot row holds one env's whole state, bytes_per_env bytes (a multiple of 16): one segment per state array, in the
+ * order of the list below, each starting 16-byte aligned, zero padding behind it. HIST is the observation history's
+ * frame ring [H, n_agents*obs_dim], empty when history = 1. Element types: fp64, except START_ROW int64, STEPS and
+ * NR_ITERS int32, EPISODE uint32.
+ * mapdn_snapshot_layout: off[s] = byte offset of segment s in a row, off[MAPDN_N_SNAPSHOT] = bytes_per_env. The layout
+ * depends on the net and on the handle's current history (mapdn_set_history): a row can only be restored into a handle
+ * whose layout is the same.
+ * mapdn_snapshot: row k of buf_dev (at buf_dev + k * bytes_per_env) receives the state of env idx_dev[k];
+ * mapdn_restore: env idx_dev[k] receives row k. idx_dev: int32 [n] on the device, or NULL for all envs in order (then n
+ * must equal the batch). Entries outside [0, batch) are skipped (nothing read or written for them). Duplicate entries in
+ * a restore list are a caller error: the result is undefined. buf_dev must be 16-byte aligned. One launch each,
+ * stream-ordered, no host synchronisation. Both refuse a null handle or buffer, n <= 0, n > batch, idx_dev = NULL with
+ * n != batch and a handle without a profile store.
+ * Noise. The Philox streams of the noise are keyed by the seed, the global env id (env_id_offset + slot), the episode
+ * counter and the step. The counter and the step are state; the seed and the global id are not. So restoring an env's
+ * own row into a slot with the same global id (on any handle with the same seed, in any process) replays its future bit
+ * for bit under the same actions. A row restored into a slot with another global id (a fork) draws that slot's noise:
+ * the first step after the fork still gives the source's reward, info and power flow (its profile row was drawn before
+ * the snapshot), the rows drawn after differ unless add_noise = 0.
+ */
+#define MAPDN_N_SNAPSHOT 15   /* segments: CUR_PL, CUR_QL, CUR_PV, CUR_Q, RES_VM, RES_VA, RES_P, RES_Q, RES_PL,
+                                 SUM_REWARDS, START_ROW, STEPS, EPISODE, NR_ITERS, HIST (empty when history = 1) */
+mapdn_status mapdn_snapshot_layout(const mapdn_env* env, int64_t* off /*[MAPDN_N_SNAPSHOT + 1]; last = bytes_per_env*/);
+mapdn_status mapdn_snapshot(mapdn_env* env, const int32_t* idx_dev /*[n] or NULL*/, int32_t n, void* buf_dev,
+                            void* stream);
+mapdn_status mapdn_restore(mapdn_env* env, const int32_t* idx_dev /*[n] or NULL*/, int32_t n, const void* buf_dev,
+                           void* stream);
+
 mapdn_status mapdn_get_obs(mapdn_env* env, double* obs_dev, void* stream);      /* :232-316 */
 mapdn_status mapdn_get_state(mapdn_env* env, double* state_dev, void* stream);  /* :213-230 */
 mapdn_status mapdn_get_field(mapdn_env* env, int32_t field, double* out_dev, void* stream);

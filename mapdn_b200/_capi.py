@@ -82,6 +82,8 @@ SIGNATURES = dict(
     mapdn_record=([_vp, _vp, _i64, _vp], _i32), mapdn_set_history=([_vp, _i32], _i32),
     mapdn_step_stacked=(_STEP[:-1] + [_vp, _vp, _i64, _vp], _i32), mapdn_get_obs_stacked=([_vp] * 3, _i32),
     mapdn_step_autoreset=(_STEP[:-1] + [_vp] * 5, _i32),
+    mapdn_snapshot_layout=([_vp] * 2, _i32), mapdn_snapshot=([_vp, _vp, _i32, _vp, _vp], _i32),
+    mapdn_restore=([_vp, _vp, _i32, _vp, _vp], _i32),
     mapdn_get_obs=([_vp] * 3, _i32), mapdn_get_state=([_vp] * 3, _i32),
     mapdn_get_field=([_vp, _i32, _vp, _vp], _i32), mapdn_solve=([_vp, _i32] + [_vp] * 12, _i32),
     mapdn_droop=([_vp, _i32] + [_vp] * 5 + [C.c_double, C.c_double, _i32] + [_vp] * 5, _i32),
@@ -89,6 +91,10 @@ SIGNATURES = dict(
 EXPORTS = tuple(SIGNATURES)
 # tester record row blocks, in the reference tester's key order (utilities/tester.py:26-32); mapdn_record_layout
 RECORD_KEYS = ("pv_active", "pv_reactive", "bus_active", "bus_reactive", "bus_voltage", "line_loss")
+# env state snapshot row segments, in the order of MAPDN_N_SNAPSHOT (mapdn_snapshot_layout) and their element types
+SNAPSHOT_SEGMENTS = ("cur_pl", "cur_ql", "cur_pv", "cur_q", "res_vm", "res_va", "res_p", "res_q", "res_pl", "sum_rewards",
+                     "start_row", "steps", "episode", "nr_iters", "hist")
+SNAPSHOT_DTYPES = dict(start_row=np.int64, steps=np.int32, episode=np.uint32, nr_iters=np.int32)   # the others: fp64
 
 _lib: Optional[C.CDLL] = None
 

@@ -189,6 +189,51 @@ __global__ void record_kernel(const __grid_constant__ Params p) {
   p.record[static_cast<size_t>(env) * p.record_stride + k] = v;
 }
 
+// ---- env state snapshots (mapdn_snapshot / mapdn_restore) ----
+// Segment s of the state: env b's bytes[s] bytes at base[s] + b * bytes[s]. A snapshot row packs the segments in the
+// order of the header's list, segment s at row offset off[s] (16-byte aligned); off[MAPDN_N_SNAPSHOT] is the row size.
+struct SnapLayout {
+  unsigned char* base[MAPDN_N_SNAPSHOT];
+  int bytes[MAPDN_N_SNAPSHOT];
+  long long off[MAPDN_N_SNAPSHOT + 1];
+};
+
+// One segment of one row by one warp, in T-wide pieces (bytes and the padded length are multiples of sizeof(T)). The
+// snapshot direction also zeroes the padding, so that equal states give equal rows.
+template <class T, bool RESTORE>
+__device__ __forceinline__ void copy_segment(unsigned char* state, unsigned char* row, int bytes, int padded, int lane) {
+  T* __restrict__ st = reinterpret_cast<T*>(state);      // a row never overlaps the state: loads may run ahead of stores
+  T* __restrict__ rw = reinterpret_cast<T*>(row);
+  const int n = bytes / static_cast<int>(sizeof(T));
+  if (RESTORE) {
+    for (int i = lane; i < n; i += 32) st[i] = rw[i];
+  } else {
+    for (int i = lane; i < n; i += 32) rw[i] = st[i];
+    for (int i = n + lane; i < padded / static_cast<int>(sizeof(T)); i += 32) rw[i] = T{};
+  }
+}
+
+// Gather (state -> rows) or scatter (RESTORE: rows -> state). Warp w moves segment w mod MAPDN_N_SNAPSHOT of row
+// k = w / MAPDN_N_SNAPSHOT between env idx[k] (env k without a list) and buf + k * off[MAPDN_N_SNAPSHOT]: 16-byte accesses
+// when the segment's size per env is a multiple of 16 (its start in the state array is then 16-byte aligned too), else
+// 8- or 4-byte ones. A row whose env is outside [0, nb) is skipped.
+template <bool RESTORE>
+__global__ void snapshot_kernel(const __grid_constant__ SnapLayout sl, const int* __restrict__ idx, int n, int nb,
+                                unsigned char* __restrict__ buf) {
+  const long long w = (blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x) >> 5;
+  const int lane = static_cast<int>(threadIdx.x & 31);
+  if (w >= static_cast<long long>(n) * MAPDN_N_SNAPSHOT) return;
+  const int k = static_cast<int>(w / MAPDN_N_SNAPSHOT), s = static_cast<int>(w - static_cast<long long>(k) * MAPDN_N_SNAPSHOT);
+  const int env = idx ? __ldg(idx + k) : k;
+  if (env < 0 || env >= nb) return;
+  const int bytes = sl.bytes[s], padded = static_cast<int>(sl.off[s + 1] - sl.off[s]);
+  unsigned char* state = sl.base[s] + static_cast<size_t>(env) * bytes;
+  unsigned char* row = buf + static_cast<size_t>(k) * sl.off[MAPDN_N_SNAPSHOT] + sl.off[s];
+  if (bytes % 16 == 0) copy_segment<int4, RESTORE>(state, row, bytes, padded, lane);
+  else if (bytes % 8 == 0) copy_segment<long long, RESTORE>(state, row, bytes, padded, lane);
+  else copy_segment<int, RESTORE>(state, row, bytes, padded, lane);
+}
+
 }  // namespace mapdn
 
 using namespace mapdn;
@@ -412,6 +457,38 @@ mapdn_status gather(mapdn_env* e, Kernel kernel, long long n, void* stream, Args
   MAPDN_CUDA(cudaGetLastError());
   e->launches++;
   return MAPDN_OK;
+}
+
+// The snapshot segments of the handle's state arrays, in the header's order (MAPDN_N_SNAPSHOT): the ring only with history
+SnapLayout snapshot_layout(const mapdn_env* e) {
+  const Params& p = e->base;
+  const long long n = p.n_bus, ng = p.n_sgen, nl = p.n_load;
+  void* const base[MAPDN_N_SNAPSHOT] = {p.cur_pl, p.cur_ql, p.cur_pv, p.cur_q, p.res_vm, p.res_va, p.res_p, p.res_q,
+                                        p.res_pl, p.sum_rewards, p.start_row, p.steps, p.episode, p.nr_iters, p.hist};
+  const long long bytes[MAPDN_N_SNAPSHOT] = {8 * nl, 8 * nl, 8 * ng, 8 * ng, 8 * n, 8 * n, 8 * n, 8 * n, 8LL * p.n_line,
+                                             8, 8, 4, 4, 4, p.history > 1 ? 8LL * p.history * ng * p.obs_dim : 0};
+  SnapLayout sl{};
+  for (int s = 0; s < MAPDN_N_SNAPSHOT; ++s) {
+    sl.base[s] = static_cast<unsigned char*>(base[s]);
+    sl.bytes[s] = static_cast<int>(bytes[s]);
+    sl.off[s + 1] = sl.off[s] + (bytes[s] + 15) / 16 * 16;
+  }
+  return sl;
+}
+
+// mapdn_snapshot / mapdn_restore: the argument checks of both, then one snapshot_kernel launch (one warp per row and
+// segment)
+mapdn_status snapshot_copy(mapdn_env* e, const int32_t* idx, int32_t n, const void* buf, void* stream, bool restore) {
+  if (!e || !buf) return fail(MAPDN_ERR_INVALID, "null argument");
+  if (!e->base.prof_pv) return fail(MAPDN_ERR_INVALID, "handle was created without a profile store");
+  if (n <= 0 || n > e->base.nb) return fail(MAPDN_ERR_INVALID, "n must be in [1, batch]");
+  if (!idx && n != e->base.nb) return fail(MAPDN_ERR_INVALID, "without an index list n must equal the batch");
+  if (reinterpret_cast<uintptr_t>(buf) % 16 != 0) return fail(MAPDN_ERR_INVALID, "snapshot buffer not 16-byte aligned");
+  const SnapLayout sl = snapshot_layout(e);
+  unsigned char* rows = static_cast<unsigned char*>(const_cast<void*>(buf));
+  const long long threads = 32LL * MAPDN_N_SNAPSHOT * n;
+  return restore ? gather(e, snapshot_kernel<true>, threads, stream, sl, idx, n, e->base.nb, rows)
+                 : gather(e, snapshot_kernel<false>, threads, stream, sl, idx, n, e->base.nb, rows);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1553,6 +1630,21 @@ mapdn_status mapdn_get_obs_stacked(mapdn_env* e, double* obs_stacked_dev, void* 
   p.obs_stacked = obs_stacked_dev;
   const long long pieces = static_cast<long long>(p.nb) * stacked_row_len(e) / ((p.obs_dim & 1) == 0 ? 2 : 1);
   return gather(e, obs_stacked_kernel, pieces, stream, p);
+}
+
+mapdn_status mapdn_snapshot_layout(const mapdn_env* e, int64_t* off) {
+  if (!e || !off) return fail(MAPDN_ERR_INVALID, "null argument");
+  const SnapLayout sl = snapshot_layout(e);
+  for (int s = 0; s <= MAPDN_N_SNAPSHOT; ++s) off[s] = sl.off[s];
+  return MAPDN_OK;
+}
+
+mapdn_status mapdn_snapshot(mapdn_env* e, const int32_t* idx_dev, int32_t n, void* buf_dev, void* stream) {
+  return snapshot_copy(e, idx_dev, n, buf_dev, stream, false);
+}
+
+mapdn_status mapdn_restore(mapdn_env* e, const int32_t* idx_dev, int32_t n, const void* buf_dev, void* stream) {
+  return snapshot_copy(e, idx_dev, n, buf_dev, stream, true);
 }
 
 mapdn_status mapdn_step_host(mapdn_env* e, const double* actions_host, int32_t add_noise, double* reward_host,

@@ -12,6 +12,7 @@ There is no CPU fallback: both classes need the CUDA library and a GPU.
 from __future__ import annotations
 
 import ctypes as C
+import hashlib
 from collections import namedtuple
 from typing import Optional
 
@@ -22,7 +23,7 @@ from . import _capi
 from ._capi import INFO_KEYS, MapdnError
 from .network import NetDesc, ProfileDesc
 
-__all__ = ["BatchedVoltageControl", "VoltageControl", "ActionSpace", "DEFAULT_ENV_ARGS", "INFO_KEYS"]
+__all__ = ["BatchedVoltageControl", "EnvSnapshot", "VoltageControl", "ActionSpace", "DEFAULT_ENV_ARGS", "INFO_KEYS"]
 
 # reference args/env_args/var_voltage_control.yaml:3-20
 DEFAULT_ENV_ARGS = dict(voltage_barrier_type="l1", voltage_weight=1.0, q_weight=0.1, line_weight=None,
@@ -46,6 +47,95 @@ class ActionSpace(object):
 
 def _ptr(t: Optional[torch.Tensor]):
     return None if t is None else C.c_void_p(t.data_ptr())
+
+
+# mapdn_cfg fields that only place the envs (batch, global id of env 0) or change the last bits (lanes per env)
+_PLACEMENT_FIELDS = ("batch", "env_id_offset", "lanes_per_env")
+
+
+def snapshot_fingerprint(net: NetDesc, profiles: Optional[ProfileDesc], env_args: dict, history: int = 1,
+                         tol: float = 0.0, max_iter: int = 0) -> str:
+    """sha256 (hex) of what the dynamics of an env depend on: the net and profile arrays as ``mapdn_create`` receives
+    them, every ``mapdn_cfg`` field except batch, env_id_offset and lanes_per_env (barrier, weights, voltage limits,
+    episode_limit, action range, reset_action, seed, state_space, tol and max_iter with their defaults filled in) and the
+    observation history. A snapshot restores only into an env with the same fingerprint."""
+    h = hashlib.sha256()
+
+    def put(tag, v):
+        h.update(tag.encode() + b"=")
+        if v is None:
+            h.update(b"none;")
+        elif isinstance(v, np.ndarray):
+            a = np.ascontiguousarray(v)
+            h.update(f"{a.dtype.str}{a.shape};".encode())
+            h.update(memoryview(a).cast("B"))
+        elif isinstance(v, float):
+            h.update(v.hex().encode() + b";")
+        else:
+            h.update(repr(v).encode() + b";")
+
+    for k in ("n_bus", "base_mva", "slack_bus", "slack_vm", "slack_va_deg"):
+        put(k, getattr(net, k))
+    put("vm_init", None if net.vm_init is None else float(net.vm_init))
+    nd, keep = _capi.make_net_desc(net)
+    for i, a in enumerate(keep):
+        put(f"net{i}", a)
+    del nd
+    if profiles is None:
+        put("profiles", None)
+    else:
+        put("rows", (profiles.n_rows, profiles.steps_per_hour, profiles.n_days))
+        for i, a in enumerate(_capi.make_profile_desc(profiles)[1]):
+            put(f"prof{i}", a)
+    cfg = _capi.make_cfg(env_args, 1, 0, 0, tol, max_iter)
+    cfg.tol = cfg.tol if cfg.tol > 0 else 1e-8                       # the defaults mapdn_create fills in
+    cfg.max_iter = cfg.max_iter if cfg.max_iter > 0 else 10
+    for name, _ in cfg._fields_:
+        if name not in _PLACEMENT_FIELDS:
+            put(name, getattr(cfg, name))
+    put("history", int(history))
+    return h.hexdigest()
+
+
+class EnvSnapshot:
+    """The device state of ``n`` envs of a :class:`BatchedVoltageControl` (``mapdn_snapshot``).
+
+    * ``data``: uint8 ``[n, bytes_per_env]`` on the env's device, one row per env (:meth:`segment` decodes it);
+    * ``env_ids``: int64 ``[n]`` (CPU) global ids of the envs the rows came from (``env_id_offset + slot``);
+    * ``layout``: the segment offsets of a row (``mapdn_snapshot_layout``, last = bytes_per_env);
+    * ``history`` and ``fingerprint`` of the env (:func:`snapshot_fingerprint`).
+
+    :meth:`state_dict` holds only tensors and plain Python values, so a checkpoint with it loads with
+    ``torch.load(weights_only=True)``."""
+
+    def __init__(self, data: torch.Tensor, env_ids: torch.Tensor, layout, history: int, fingerprint: str):
+        self.data, self.env_ids = data, env_ids.to(torch.int64).cpu()
+        self.layout, self.history, self.fingerprint = [int(x) for x in layout], int(history), str(fingerprint)
+        if data.dtype != torch.uint8 or data.dim() != 2 or data.shape[0] != self.env_ids.numel():
+            raise ValueError(f"snapshot data must be uint8 [n, bytes_per_env] with n = len(env_ids), got "
+                             f"{data.dtype} {tuple(data.shape)} for {self.env_ids.numel()} ids")
+
+    def __len__(self):
+        return int(self.env_ids.numel())
+
+    def state_dict(self) -> dict:
+        return dict(data=self.data, env_ids=self.env_ids, layout=list(self.layout), history=self.history,
+                    fingerprint=self.fingerprint)
+
+    @classmethod
+    def from_state_dict(cls, d: dict) -> "EnvSnapshot":
+        return cls(d["data"], d["env_ids"], d["layout"], d["history"], d["fingerprint"])
+
+    def segment(self, name: str, count: int) -> torch.Tensor:
+        """Segment ``name`` (``_capi.SNAPSHOT_SEGMENTS``) of every row decoded as ``[n, count]`` of its element type;
+        ``count`` is the array's entries per env (``n_load``, ``n_sgen``, ``n_bus``, ``n_line`` of ``env.dims``, 1 for the
+        scalars, ``history * n_agents * obs_dim`` for the frame ring)."""
+        s = _capi.SNAPSHOT_SEGMENTS.index(name)
+        dt = {np.int64: torch.int64, np.int32: torch.int32, np.uint32: torch.int32}.get(
+            _capi.SNAPSHOT_DTYPES.get(name), torch.float64)
+        size = torch.empty((), dtype=dt).element_size()
+        raw = self.data[:, self.layout[s]:self.layout[s] + count * size].contiguous()
+        return raw.view(dt).reshape(len(self), count)
 
 
 class BatchedVoltageControl:
@@ -111,6 +201,9 @@ class BatchedVoltageControl:
             _capi.check(L.mapdn_set_history(h, self.history))
             self.obs_stacked = torch.zeros(B, d.n_agents, self.stacked_obs_size, dtype=f64, device=self.device)
         self._host = None
+        # what the snapshot fingerprint covers beyond the net and the profile store (computed on first use)
+        self.env_id_offset = int(env_id_offset)
+        self._cfg, self._fingerprint, self._snapshot_layout = cfg, None, None
         # raw pointers of the internal buffers (ctypes converts plain ints for c_void_p parameters): keeps the
         # per-step Python overhead of the hot call small
         self._p_obs, self._p_state = self.obs.data_ptr(), self.state.data_ptr()
@@ -358,6 +451,91 @@ class BatchedVoltageControl:
         out = torch.empty(self.batch, self.dims.get(_capi.FIELD_DIMS.get(name), 1), dtype=torch.float64, device=self.device)
         _capi.check(self._L.mapdn_get_field(self._h, _capi.FIELDS[name], _ptr(out), self._stream()))
         return out
+
+    # ---- env state snapshots (mapdn_snapshot / mapdn_restore) ----------------------------------------
+    @property
+    def fingerprint(self) -> str:
+        """:func:`snapshot_fingerprint` of this env, computed on first use (it hashes the whole profile store)."""
+        if self._fingerprint is None:
+            c = self._cfg
+            self._fingerprint = snapshot_fingerprint(self.net, self.profiles, self.args, self.history, c.tol, c.max_iter)
+        return self._fingerprint
+
+    @property
+    def snapshot_layout(self):
+        """Byte offsets of the ``MAPDN_N_SNAPSHOT`` segments of a snapshot row, then bytes_per_env."""
+        if self._snapshot_layout is None:
+            off = (C.c_int64 * (len(_capi.SNAPSHOT_SEGMENTS) + 1))()
+            _capi.check(self._L.mapdn_snapshot_layout(self._h, off))
+            self._snapshot_layout = [int(x) for x in off]
+        return self._snapshot_layout
+
+    def _slots(self, idx, what: str, unique: bool) -> torch.Tensor:
+        """``idx`` as an int64 CPU tensor of slots in [0, batch), checked on the host (a CUDA tensor costs one sync)."""
+        t = torch.as_tensor(idx).reshape(-1)
+        if t.dtype.is_floating_point or t.dtype == torch.bool:
+            raise ValueError(f"{what}: slot indices must be integers, got {t.dtype}")
+        t = t.to("cpu", torch.int64)
+        if t.numel() == 0 or t.numel() > self.batch:
+            raise ValueError(f"{what}: need 1 to {self.batch} slots, got {t.numel()}")
+        if int(t.min()) < 0 or int(t.max()) >= self.batch:
+            raise ValueError(f"{what}: slots must be in [0, {self.batch}), got {t.min().item()}..{t.max().item()}")
+        if unique and torch.unique(t).numel() != t.numel():
+            raise ValueError(f"{what}: duplicate slots")
+        return t
+
+    def snapshot(self, idx=None) -> EnvSnapshot:
+        """The state of the envs in slots ``idx`` (all envs in order when None; repeats allowed) as an
+        :class:`EnvSnapshot` whose rows live on this env's device. One launch, stream-ordered; ``idx`` is checked on
+        the host, so a CUDA index tensor costs one sync."""
+        L = self.snapshot_layout
+        slots = torch.arange(self.batch) if idx is None else self._slots(idx, "snapshot", unique=False)
+        data = torch.empty(slots.numel(), L[-1], dtype=torch.uint8, device=self.device)
+        ids = None if idx is None else slots.to(self.device, torch.int32)
+        _capi.check(self._L.mapdn_snapshot(self._h, _ptr(ids), slots.numel(), _ptr(data), self._stream()))
+        return EnvSnapshot(data, slots + self.env_id_offset, L, self.history, self.fingerprint)
+
+    def restore(self, snap: EnvSnapshot, idx=None) -> torch.Tensor:
+        """Puts the rows of ``snap`` back and returns the slots written (int64, CPU). ``idx``: the slot of each row (no
+        repeats). Without it every row goes to the slot of its global id (``env_id - env_id_offset``) and rows of ids
+        outside this env are skipped, so a snapshot of one env of B envs restores into N shards of B / N. Refuses a
+        snapshot of an env with another fingerprint, layout or history. Then ``obs``, ``state`` and (``history > 1``)
+        ``obs_stacked`` are gathered again from the restored state, for all envs. Stream-ordered, no host sync unless
+        ``idx`` is a CUDA tensor (one)."""
+        if snap.history != self.history or snap.layout != self.snapshot_layout:
+            raise ValueError(f"restore: snapshot layout {snap.layout} (history {snap.history}) does not match this env's "
+                             f"{self.snapshot_layout} (history {self.history})")
+        if snap.fingerprint != self.fingerprint:
+            raise ValueError("restore: the snapshot comes from an env with another net, profile store or env_args")
+        data = snap.data
+        if idx is None:
+            slots = snap.env_ids - self.env_id_offset
+            rows = torch.nonzero((slots >= 0) & (slots < self.batch)).reshape(-1)
+            if rows.numel() == 0:
+                return rows
+            if rows.numel() != len(snap):
+                data, slots = data[rows.to(data.device)], slots[rows]
+            slots = self._slots(slots, "restore", unique=True)
+        else:
+            slots = self._slots(idx, "restore", unique=True)
+            if slots.numel() != len(snap):
+                raise ValueError(f"restore: {slots.numel()} slots for {len(snap)} snapshot rows")
+        data = data.to(self.device).contiguous()
+        whole = slots.numel() == self.batch and bool(torch.equal(slots, torch.arange(self.batch)))
+        ids = None if whole else slots.to(self.device, torch.int32)
+        st = self._stream()
+        _capi.check(self._L.mapdn_restore(self._h, _ptr(ids), slots.numel(), _ptr(data), st))
+        _capi.check(self._L.mapdn_get_obs(self._h, _ptr(self.obs), st))
+        _capi.check(self._L.mapdn_get_state(self._h, _ptr(self.state), st))
+        if self.history > 1:
+            _capi.check(self._L.mapdn_get_obs_stacked(self._h, _ptr(self.obs_stacked), st))
+        return slots
+
+    def fork(self, src, dst) -> torch.Tensor:
+        """Copies the state of slots ``src`` into slots ``dst`` (``restore(snapshot(src), dst)``: two launches through a
+        temporary, so ``src`` and ``dst`` may overlap). One source into K slots: ``fork([s] * K, dst)``. The copies draw
+        the noise of their own slots from the next profile row on (see the header's noise rules)."""
+        return self.restore(self.snapshot(src), dst)
 
     # ---- tester records (reference utilities/tester.py:26-55) ---------------------------------------
     @property

@@ -100,6 +100,18 @@ class DeviceTransitionBuffer:
     def clear(self):
         self.head = self.count = 0
 
+    def state_dict(self) -> dict:
+        return dict(data=dict(self.data), head=self.head, count=self.count)
+
+    def load_state_dict(self, d: dict):
+        """The fields of a :meth:`state_dict` (``value`` / ``next_value`` take the checkpoint's width)."""
+        for k in TRANSITION_FIELDS:
+            v = d["data"][k]
+            if tuple(v.shape[:2]) != (self.S, self.B):
+                raise ValueError(f"transition buffer {k}: checkpoint shape {tuple(v.shape)}, buffer [{self.S}, {self.B}, ...]")
+            self.data[k] = v.to(self.device, self.data[k].dtype).clone()
+        self.head, self.count = int(d["head"]), int(d["count"])
+
     def add(self, **fields):
         """One lock-step: every field ``[B, ...]``. The width of ``value`` / ``next_value`` is the learner's business (one
         Q per agent for most of the reference's algorithms, two for MATD3's twin critics, ``sample_size`` coalition
@@ -224,6 +236,23 @@ class BatchedMarlRunner:
         for k, v in zip(INFO_KEYS, (info_sum / denom).tolist()):
             stat["mean_train_" + k] = v
         return stat
+
+    def state_dict(self) -> dict:
+        """What the next :meth:`train_process` depends on besides the model: the env's state (its per-env episode counters
+        key the sampled starts of the next reset), the counters ``steps`` / ``episodes`` and the transition buffer.
+        Tensors and plain values only; learner weights, optimiser state and the torch RNG are the caller's, as in the
+        reference's ``train.py``."""
+        d = dict(env=self.env.snapshot().state_dict(), steps=self.steps, episodes=self.episodes)
+        if self.buffer is not None:
+            d["buffer"] = self.buffer.state_dict()
+        return d
+
+    def load_state_dict(self, d: dict):
+        from .env import EnvSnapshot
+        self.env.restore(EnvSnapshot.from_state_dict(d["env"]))
+        self.steps, self.episodes = int(d["steps"]), int(d["episodes"])
+        if self.buffer is not None and "buffer" in d:
+            self.buffer.load_state_dict(d["buffer"])
 
     @torch.no_grad()
     def evaluation(self, stat: dict, num_eval_episodes: Optional[int] = None) -> dict:

@@ -51,6 +51,19 @@ class DeviceReplayBuffer:
     def __len__(self):
         return self.count
 
+    _FIELDS = ("obs", "next_obs", "action", "reward", "done")
+
+    def state_dict(self) -> dict:
+        return dict({k: getattr(self, k) for k in self._FIELDS}, head=self.head, count=self.count)
+
+    def load_state_dict(self, d: dict):
+        for k in self._FIELDS:
+            if tuple(d[k].shape) != tuple(getattr(self, k).shape):
+                raise ValueError(f"replay buffer {k}: checkpoint shape {tuple(d[k].shape)}, "
+                                 f"buffer {tuple(getattr(self, k).shape)}")
+            getattr(self, k).copy_(d[k])
+        self.head, self.count = int(d["head"]), int(d["count"])
+
     def sample(self, batch_size: int, generator: Optional[torch.Generator] = None):
         n = min(batch_size, self.count)
         idx = torch.randperm(self.count, device=self.device, generator=generator)[:n]
@@ -115,6 +128,33 @@ class BatchedRollout:
             obs = torch.where(done.bool()[:, None, None], env.reset_obs if autoreset else env.obs, next_obs)
         self._obs = obs
         return obs.clone()
+
+    def state_dict(self) -> dict:
+        """What a later :meth:`run` continues from: the env's state (:meth:`env.snapshot`, all envs), the running
+        episode returns, the finished-episode statistics and the replay buffer. Tensors and plain values only
+        (``torch.save`` / ``torch.load(weights_only=True)``); the policy is the caller's."""
+        d = dict(env=self.env.snapshot().state_dict(), episode_return=self.episode_return, ret_ring=self._ret_ring,
+                 ret_n=self._ret_n, ret_sum=self._ret_sum, info_sum=self.info_sum, started=self._started)
+        if self.buffer is not None:
+            d["buffer"] = self.buffer.state_dict()
+        return d
+
+    def load_state_dict(self, d: dict):
+        """Restores a :meth:`state_dict` into this rollout and its env (one with the same fingerprint; any
+        ``env_id_offset`` that covers the envs). The observation the next step acts on is gathered again from the restored
+        env state (``env.get_obs()``), not stored."""
+        from .env import EnvSnapshot
+        self.env.restore(EnvSnapshot.from_state_dict(d["env"]))
+        dev = self.episode_return.device
+        for name, key in (("episode_return", "episode_return"), ("_ret_n", "ret_n"), ("_ret_sum", "ret_sum"),
+                          ("info_sum", "info_sum")):
+            setattr(self, name, d[key].to(dev).clone())
+        self._ret_ring = d["ret_ring"].to(dev).clone()
+        self.keep_returns = int(self._ret_ring.numel())
+        self._started = bool(d["started"])
+        self._obs = self.env.get_obs().clone() if self._started else None
+        if self.buffer is not None and "buffer" in d:
+            self.buffer.load_state_dict(d["buffer"])
 
     def completed_episode_returns(self) -> torch.Tensor:
         """Returns of the episodes that ended so far - the last ``keep_returns`` of them (one host sync)."""
