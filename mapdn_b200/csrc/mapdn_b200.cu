@@ -1181,6 +1181,7 @@ HotBlob build_hot_blob(const Ybus& y, const Forest& f, const Sweeps& s, const El
 struct Geometry {
   bool cold_tables = false, stage_rec = false;   // the two ways to buy shared memory, see below
   int stride2 = 0, epb = 0, smem = 0, helper_threads = 32;
+  int smem_needed = 0;                           // set on a refusal: the bytes of the smallest plan (one group of envs)
 };
 
 // ---- 5. launch geometry ----
@@ -1230,18 +1231,68 @@ mapdn_status plan_geometry(int npq, int ng, int nl, int G, int batch, int bytes_
     const int k = atoi(ov);
     if (k >= 0 && k < 4 && plans[k].ok) best = &plans[k];
   }
-  if (best) { geo.stride2 = best->st2; geo.epb = best->epb; geo.stage_rec = best->rec; geo.cold_tables = best->cold; }
-  auto smem_for = [&](int c) { return smem_with(geo.cold_tables, geo.stride2, c); };
-  if (geo.epb == 0 || smem_for(geo.epb) > max_smem)
-    return fail(MAPDN_ERR_UNSUPPORTED, "network too large for the shared-memory resident solver (" +
-                                           std::to_string(smem_for(std::max(geo.epb, unit))) + " B needed)");
-  geo.smem = static_cast<int>(smem_for(geo.epb));
+  if (!best) {       // every plan that could be built needs more than max_smem with a single group of envs
+    size_t need = SIZE_MAX;
+    for (const Plan& pl : plans) if (pl.st2 > 0) need = std::min(need, smem_with(pl.cold, pl.st2, unit));
+    geo.smem_needed = static_cast<int>(need);
+    return fail(MAPDN_ERR_UNSUPPORTED, "network too large for the shared-memory resident solver (" + std::to_string(need) +
+                                           " B needed at " + std::to_string(G) + " lanes per env, " +
+                                           std::to_string(max_smem) + " B available)");
+  }
+  geo.stride2 = best->st2; geo.epb = best->epb; geo.stage_rec = best->rec; geo.cold_tables = best->cold;
+  geo.smem = static_cast<int>(smem_with(geo.cold_tables, geo.stride2, geo.epb));
   // helper warps (next profile rows + noise, concurrent with the Newton iteration): one per 256 Box-Muller pairs of a
   // CTA round, at most 4 -- a single warp can be the critical path of case322
   const int n_pair = (ng + 2 * nl + 1) / 2;
   geo.helper_threads = 32 * std::min(4, std::max(1, (geo.epb * n_pair + kHelperPairsPerWarp - 1) / kHelperPairsPerWarp));
   if (const char* ov = getenv("MAPDN_HELPERS")) geo.helper_threads = 32 * std::min(4, std::max(1, atoi(ov)));   // tuning override
   return MAPDN_OK;
+}
+
+// Everything sections 2a to 5 plan for one lane count. relabel_nodes permutes the forest, so each plan owns a copy.
+struct LanePlan {
+  Forest f;
+  Sweeps s;
+  ObsPrograms o;
+  BranchTables t;
+  HotBlob hot;
+  Geometry geo;
+};
+
+mapdn_status plan_for_lanes(const Ybus& y, const Forest& forest, const mapdn_net_desc& net, const mapdn_cfg& cfg, int lanes,
+                            const cudaDeviceProp& dp, LanePlan& p) {
+  p.f = forest;
+  MAPDN_TRY(plan_sweeps(p.f, lanes, p.s));
+  relabel_nodes(y, p.f, p.s);
+  const ElementMaps m = element_maps(net, p.f);
+  MAPDN_TRY(obs_programs(net, p.f, p.s.G, cfg.state_space_mask, p.o));
+  p.t = branch_tables(y, p.f, net.base_mva);
+  p.hot = build_hot_blob(y, p.f, p.s, m, p.o, p.t);
+  return plan_geometry(net.n_bus - 1, net.n_sgen, net.n_load, p.s.G, cfg.batch, p.hot.bytes_core, p.hot.bytes_full,
+                       dp.sharedMemPerBlockOptin, dp.multiProcessorCount, p.geo);
+}
+
+// The lane count of the handle. An explicit lanes_per_env is planned as asked. With lanes_per_env = 0 the default of
+// plan_sweeps comes first; the schedules grow as depth x lanes, so a deep feeder (a 400-bus chain at 64 lanes) can miss
+// shared memory at the default and fit at fewer lanes. Then the other lane counts are tried in a fixed order - one warp
+// per env, narrower groups, multi-warp groups last - and the first that fits is taken. The dense fallback of a meshed
+// net always works one warp per env.
+mapdn_status plan_lanes(const Ybus& y, const Forest& forest, const mapdn_net_desc& net, const mapdn_cfg& cfg,
+                        const cudaDeviceProp& dp, LanePlan& p) {
+  const mapdn_status st = plan_for_lanes(y, forest, net, cfg, cfg.lanes_per_env, dp, p);
+  if (st != MAPDN_ERR_UNSUPPORTED || p.geo.smem_needed == 0 || cfg.lanes_per_env != 0 || forest.meshed) return st;
+  int need = p.geo.smem_needed, need_lanes = p.s.G;
+  for (const int lanes : {32, 16, 8, 4, 64, 128}) {
+    if (lanes == p.s.G) continue;
+    LanePlan q;
+    const mapdn_status sq = plan_for_lanes(y, forest, net, cfg, lanes, dp, q);
+    if (sq == MAPDN_OK) { p = std::move(q); return MAPDN_OK; }
+    if (sq != MAPDN_ERR_UNSUPPORTED || q.geo.smem_needed == 0) return sq;
+    if (q.geo.smem_needed < need) { need = q.geo.smem_needed; need_lanes = lanes; }
+  }
+  return fail(MAPDN_ERR_UNSUPPORTED, "network too large for the shared-memory resident solver at every lane count (" +
+                                         std::to_string(need) + " B needed at " + std::to_string(need_lanes) + " lanes per env, " +
+                                         std::to_string(dp.sharedMemPerBlockOptin) + " B available)");
 }
 
 // The flat start of the first Newton iteration: every PQ bus at vm_init, angle 0; the slack at vm0, va0 = e0 + j f0
@@ -1489,32 +1540,23 @@ mapdn_status mapdn_create(const mapdn_net_desc* net, const mapdn_profile_desc* p
   if (!e) return fail(MAPDN_ERR_NOMEM, "out of host memory");
   e->device = device;
   e->cfg = *cfg;
-  const int n = net->n_bus, nl = net->n_load, ng = net->n_sgen;
+  const int n = net->n_bus;
 
   Ybus y;
   MAPDN_TRY(ybus_on_device(e.get(), *net, y));
-  Forest f;
-  MAPDN_TRY(build_forest(y, n, net->slack_bus, f));
-  Sweeps s;
-  MAPDN_TRY(plan_sweeps(f, cfg->lanes_per_env, s));
-  relabel_nodes(y, f, s);
-  const ElementMaps m = element_maps(*net, f);
-  ObsPrograms o;
-  MAPDN_TRY(obs_programs(*net, f, s.G, cfg->state_space_mask, o));
-  const BranchTables t = branch_tables(y, f, net->base_mva);
-  const HotBlob hot = build_hot_blob(y, f, s, m, o, t);
+  Forest forest;
+  MAPDN_TRY(build_forest(y, n, net->slack_bus, forest));
   cudaDeviceProp dp{};
   MAPDN_CUDA(cudaGetDeviceProperties(&dp, device));
-  Geometry geo;
-  MAPDN_TRY(plan_geometry(n - 1, ng, nl, s.G, cfg->batch, hot.bytes_core, hot.bytes_full, dp.sharedMemPerBlockOptin,
-                          dp.multiProcessorCount, geo));
+  LanePlan p;
+  MAPDN_TRY(plan_lanes(y, forest, *net, *cfg, dp, p));
   const FlatStart v0 = flat_start(*net);
-  const std::vector<double> ft = first_iteration_factors(f, hot, v0);
+  const std::vector<double> ft = first_iteration_factors(p.f, p.hot, v0);
 
-  e->dense = f.meshed;
-  e->G = s.G; e->threads = geo.epb * s.G; e->epb = geo.epb; e->smem = geo.smem; e->helper_threads = geo.helper_threads;
+  e->dense = p.f.meshed;
+  e->G = p.s.G; e->threads = p.geo.epb * p.s.G; e->epb = p.geo.epb; e->smem = p.geo.smem; e->helper_threads = p.geo.helper_threads;
   MAPDN_TRY(size_kernels(e.get(), dp));
-  MAPDN_TRY(upload_plan(e.get(), *net, prof, y, f, s, o, t, hot, geo, v0, ft));
+  MAPDN_TRY(upload_plan(e.get(), *net, prof, y, p.f, p.s, p.o, p.t, p.hot, p.geo, v0, ft));
   // the memsets / uploads above ran on the legacy default stream: order them before any launch of the caller's
   // (possibly non-blocking) streams
   MAPDN_CUDA(cudaDeviceSynchronize());
