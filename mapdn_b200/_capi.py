@@ -128,9 +128,10 @@ def lib() -> C.CDLL:
     return L
 
 
-def check(status: int):
+def check(status: int, L: C.CDLL):
+    """Raises MapdnError with the error text of ``L``, the library that returned ``status``, unless it is 0."""
     if status != 0:
-        raise MapdnError(f"mapdn status {status}: {lib().mapdn_last_error().decode()}")
+        raise MapdnError(f"mapdn status {status}: {L.mapdn_last_error().decode()}")
 
 
 def _p(a: Optional[np.ndarray], typ):

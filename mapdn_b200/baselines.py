@@ -49,7 +49,7 @@ def no_control(env, p_load, q_load, p_pv):
 
 
 def droop_control(env, p_load, q_load, p_pv, s_rated, q_max_manual=None, max_ite=100, gain=0.1, tol=1e-4):
-    """Batched droop control, one launch. ``p_load/q_load [B, n_load]``, ``p_pv [B, n_sgen]`` CUDA fp64;
+    """Batched droop control, one launch. ``p_load/q_load [B, n_load]``, ``p_pv [B, n_sgen]`` fp64 on ``env.device``;
     ``s_rated [n_sgen]`` (= 1.2 * max PV in the reference). Returns dict(vm, q, loss, iterations) where ``q`` is the
     reactive power of the last power flow (``result.gen(:,3)`` in the script) and ``iterations`` the number of power
     flows run per env."""
@@ -68,7 +68,7 @@ def droop_control(env, p_load, q_load, p_pv, s_rated, q_max_manual=None, max_ite
     ptr = lambda x: C.c_void_p(x.data_ptr())
     _capi.check(env._L.mapdn_droop(env._h, B, ptr(p_load), ptr(q_load), ptr(p_pv), ptr(s_rated), ptr(q_max_manual),
                                    float(gain), float(tol), int(max_ite), ptr(vm), ptr(q), ptr(loss), ptr(iters),
-                                   env._stream()))
+                                   env._stream()), env._L)
     return dict(vm=vm, q=q, loss=loss, iterations=iters)
 
 

@@ -7,7 +7,8 @@
   same method names, argument meaning and return shapes (PyMARL ``MultiAgentEnv`` API,
   reference ``environments/multiagentenv.py``).
 
-There is no CPU fallback: both classes need the CUDA library and a GPU.
+There is no CPU fallback: by default both classes bind the CUDA library and need a GPU. ``BatchedVoltageControl(...,
+library=L, device="cpu")`` binds another build of the C-ABI whose device memory is host memory.
 """
 from __future__ import annotations
 
@@ -143,12 +144,18 @@ class BatchedVoltageControl:
 
     ``env_args``: dict with the keys of the reference's ``env_args`` (DEFAULT_ENV_ARGS).
     ``env_id_offset``: global id of env 0 (multi-GPU sharding keeps the RNG streams per env id).
+    ``library``: the C-ABI library to bind (``ctypes.CDLL`` with ``_capi.bind`` applied), ``_capi.lib()`` when None.
+    ``device="cpu"`` needs one whose "device" memory is host memory (such as a build of the kernel source for a CPU
+    emulation of CUDA): the tensors are then CPU tensors, host buffers are not pinned and no stream is passed.
     """
 
     def __init__(self, net: NetDesc, profiles: Optional[ProfileDesc], env_args: Optional[dict] = None,
                  batch: int = 1, device: Optional[int] = None, env_id_offset: int = 0,
-                 lanes_per_env: int = 0, tol: float = 0.0, max_iter: int = 0):
-        if not torch.cuda.is_available():
+                 lanes_per_env: int = 0, tol: float = 0.0, max_iter: int = 0, library: Optional[C.CDLL] = None):
+        self._cpu = str(device) == "cpu"
+        if self._cpu and library is None:
+            raise MapdnError("device='cpu' needs a library whose device memory is host memory (there is no CPU fallback)")
+        if not self._cpu and not torch.cuda.is_available():
             raise MapdnError("mapdn_b200 needs a CUDA device (there is no CPU fallback)")
         args = dict(DEFAULT_ENV_ARGS)
         args.update(env_args or {})
@@ -163,9 +170,12 @@ class BatchedVoltageControl:
         self.args = args
         self.net, self.profiles = net, profiles
         self.batch = int(batch)
-        self.device_index = torch.cuda.current_device() if device is None else int(device)
-        self.device = torch.device("cuda", self.device_index)
-        L = _capi.lib()
+        if self._cpu:
+            self.device_index, self.device = 0, torch.device("cpu")
+        else:
+            self.device_index = torch.cuda.current_device() if device is None else int(device)
+            self.device = torch.device("cuda", self.device_index)
+        L = _capi.lib() if library is None else library
         cfg = _capi.make_cfg(args, self.batch, env_id_offset, lanes_per_env, tol, max_iter)
         if args["line_weight"] is None and args["q_weight"] is None:
             raise NotImplementedError("Please at least give one weight, either q_weight or line_weight.")
@@ -173,11 +183,11 @@ class BatchedVoltageControl:
         pd_, keep2 = (None, None) if profiles is None else _capi.make_profile_desc(profiles)
         h = C.c_void_p()
         _capi.check(L.mapdn_create(C.byref(nd), None if pd_ is None else C.byref(pd_), C.byref(cfg),
-                                   self.device_index, C.byref(h)))
+                                   self.device_index, C.byref(h)), L)
         del keep1, keep2
         self._h, self._L = h, L
         d = _capi.DimsC()
-        _capi.check(L.mapdn_get_dims(h, C.byref(d)))
+        _capi.check(L.mapdn_get_dims(h, C.byref(d)), L)
         self.dims = {k: getattr(d, k) for k, _ in d._fields_}
         self.n_agents, self.n_actions = d.n_agents, d.n_actions
         self.obs_size, self.state_size = d.obs_dim, d.state_dim
@@ -186,19 +196,18 @@ class BatchedVoltageControl:
                                         high=args["action_scale"] + args["action_bias"])
         self.s_max = None if profiles is None else profiles.s_max
         B, f64 = self.batch, torch.float64
-        with torch.cuda.device(self.device):
-            self.obs = torch.zeros(B, d.n_agents, d.obs_dim, dtype=f64, device=self.device)
-            self.state = torch.zeros(B, d.state_dim, dtype=f64, device=self.device)
-            self.reward = torch.zeros(B, dtype=f64, device=self.device)
-            self.terminated = torch.zeros(B, dtype=torch.uint8, device=self.device)
-            self.info = torch.zeros(B, len(INFO_KEYS), dtype=f64, device=self.device)
-            self.reset_ok = torch.ones(B, dtype=torch.uint8, device=self.device)
+        self.obs = torch.zeros(B, d.n_agents, d.obs_dim, dtype=f64, device=self.device)
+        self.state = torch.zeros(B, d.state_dim, dtype=f64, device=self.device)
+        self.reward = torch.zeros(B, dtype=f64, device=self.device)
+        self.terminated = torch.zeros(B, dtype=torch.uint8, device=self.device)
+        self.info = torch.zeros(B, len(INFO_KEYS), dtype=f64, device=self.device)
+        self.reset_ok = torch.ones(B, dtype=torch.uint8, device=self.device)
         # history > 1 (reference :303-315): the step kernel keeps a ring of the last frames and writes the stacked rows
         # [B, n_agents, history * obs_dim] here; a learner is sized with stacked_obs_size
         self.stacked_obs_size = self.history * self.obs_size
         self.obs_stacked = self.obs
         if self.history > 1:
-            _capi.check(L.mapdn_set_history(h, self.history))
+            _capi.check(L.mapdn_set_history(h, self.history), L)
             self.obs_stacked = torch.zeros(B, d.n_agents, self.stacked_obs_size, dtype=f64, device=self.device)
         self._host = None
         # what the snapshot fingerprint covers beyond the net and the profile store (computed on first use)
@@ -223,7 +232,8 @@ class BatchedVoltageControl:
             pass
 
     def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        """Handle of the device's current stream (None on the CPU device); ctypes converts both for a c_void_p."""
+        return None if self._cpu else torch.cuda.current_stream(self.device).cuda_stream
 
     def _chk(self, t: torch.Tensor, shape, dtype=torch.float64, name="tensor"):
         if t.device != self.device or t.dtype != dtype or tuple(t.shape) != tuple(shape) or not t.is_contiguous():
@@ -252,7 +262,7 @@ class BatchedVoltageControl:
             self._chk(mask, (self.batch,), torch.uint8, "mask")
         p_state = _ptr(self.state) if want_state else None          # rollouts that never read get_state skip it
         _capi.check(self._L.mapdn_reset(self._h, _ptr(start), _ptr(mask), int(add_noise), _ptr(self.obs),
-                                        p_state, _ptr(self.reset_ok), self._stream()))
+                                        p_state, _ptr(self.reset_ok), self._stream()), self._L)
         if check:
             sel = torch.ones_like(self.reset_ok) if mask is None else mask
             for _ in range(max_retries + 1):
@@ -262,15 +272,15 @@ class BatchedVoltageControl:
                 if start is not None:
                     raise MapdnError("manual_reset: the power flow of the requested start does not converge")
                 _capi.check(self._L.mapdn_reset(self._h, None, _ptr(bad), int(add_noise), _ptr(self.obs),
-                                                p_state, _ptr(self.reset_ok), self._stream()))
+                                                p_state, _ptr(self.reset_ok), self._stream()), self._L)
                 sel = bad
             else:
                 raise MapdnError(f"reset: {int(bad.sum())} env(s) found no solvable start in "
                                  f"{16 * (max_retries + 1)} draws")
         if mask is not None and want_state:   # state of the untouched envs
-            _capi.check(self._L.mapdn_get_state(self._h, _ptr(self.state), self._stream()))
+            _capi.check(self._L.mapdn_get_state(self._h, _ptr(self.state), self._stream()), self._L)
         if self.history > 1:
-            _capi.check(self._L.mapdn_get_obs_stacked(self._h, _ptr(self.obs_stacked), self._stream()))
+            _capi.check(self._L.mapdn_get_obs_stacked(self._h, _ptr(self.obs_stacked), self._stream()), self._L)
         return self.obs, self.state
 
     def step(self, actions: torch.Tensor, add_noise: bool = True, want_obs: bool = True, want_info: bool = True,
@@ -285,7 +295,7 @@ class BatchedVoltageControl:
         if (actions.dtype is not torch.float64 or tuple(actions.shape) != self._act_shape or actions.device != self.device
                 or not actions.is_contiguous()):
             self._chk(actions, self._act_shape, name="actions")
-        stream = torch.cuda.current_stream(self.device).cuda_stream
+        stream = self._stream()
         if self.history > 1:
             st = self._L.mapdn_step_stacked(self._h, actions.data_ptr(), int(add_noise), self._p_reward, self._p_term,
                                             self._p_info if want_info else None, self._p_obs if want_obs else None,
@@ -300,7 +310,7 @@ class BatchedVoltageControl:
             st = self._L.mapdn_step(self._h, actions.data_ptr(), int(add_noise), self._p_reward, self._p_term,
                                     self._p_info if want_info else None, self._p_obs if want_obs else None, stream)
         if st:
-            _capi.check(st)
+            _capi.check(st, self._L)
         return self.reward, self.terminated, self.info
 
     def step_autoreset(self, actions: torch.Tensor, add_noise: bool = True):
@@ -324,15 +334,15 @@ class BatchedVoltageControl:
         st = self._L.mapdn_step_autoreset(self._h, actions.data_ptr(), int(add_noise), self._p_reward, self._p_term,
                                           self._p_info, self._p_obs, self.obs_stacked.data_ptr() if hist else None,
                                           self.reset_obs.data_ptr(), self.reset_obs_stacked.data_ptr() if hist else None,
-                                          self.reset_ok.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream)
+                                          self.reset_ok.data_ptr(), self._stream())
         if st:
-            _capi.check(st)
+            _capi.check(st, self._L)
         return self.reward, self.terminated, self.info
 
     # host-buffer path (what a CPU-side caller such as the reference trainer pays end to end)
     def _host_buffers(self):
         if self._host is None:
-            B, pin = self.batch, dict(pin_memory=True)
+            B, pin = self.batch, dict(pin_memory=not self._cpu)
             self._host = dict(
                 actions=torch.zeros(B, self.n_agents, dtype=torch.float64, **pin),
                 reward=torch.zeros(B, dtype=torch.float64, **pin),
@@ -361,17 +371,18 @@ class BatchedVoltageControl:
         hb = self._host_buffers()
         hb["actions"].numpy()[...] = actions
         f32 = np.dtype(obs_dtype) == np.float32
-        stream = torch.cuda.current_stream(self.device).cuda_stream
+        stream = self._stream()
         if layout == "compact":
             row = self.obs_row_len
             key = "obs_c32" if f32 else "obs_c"
             if key not in hb:
-                hb[key] = torch.zeros(self.batch, row, dtype=torch.float32 if f32 else torch.float64).pin_memory()
+                hb[key] = torch.zeros(self.batch, row, dtype=torch.float32 if f32 else torch.float64,
+                                      pin_memory=not self._cpu)
             obs = hb[key]
             _capi.check(self._L.mapdn_step_host_compact(self._h, hb["actions"].data_ptr(), int(add_noise),
                                                         hb["reward"].data_ptr(), hb["terminated"].data_ptr(),
                                                         hb["info"].data_ptr(), obs.data_ptr(), int(f32),
-                                                        int(staged is False), int(sync), stream))
+                                                        int(staged is False), int(sync), stream), self._L)
             return hb["reward"].numpy(), hb["terminated"].numpy(), hb["info"].numpy(), obs.numpy()
         if layout != "padded":
             raise ValueError("layout must be 'padded' or 'compact'")
@@ -379,23 +390,24 @@ class BatchedVoltageControl:
         if staged:
             fn = self._L.mapdn_step_host_f32obs if f32 else self._L.mapdn_step_host
             _capi.check(fn(self._h, hb["actions"].data_ptr(), int(add_noise), hb["reward"].data_ptr(),
-                           hb["terminated"].data_ptr(), hb["info"].data_ptr(), obs.data_ptr(), stream))
+                           hb["terminated"].data_ptr(), hb["info"].data_ptr(), obs.data_ptr(), stream), self._L)
         else:
             _capi.check(self._L.mapdn_step_host_pinned(self._h, hb["actions"].data_ptr(), int(add_noise),
                                                        hb["reward"].data_ptr(), hb["terminated"].data_ptr(),
-                                                       hb["info"].data_ptr(), obs.data_ptr(), int(f32), 1, int(sync), stream))
+                                                       hb["info"].data_ptr(), obs.data_ptr(), int(f32), 1, int(sync),
+                                                       stream), self._L)
         return hb["reward"].numpy(), hb["terminated"].numpy(), hb["info"].numpy(), obs.numpy()
 
     def wait(self):
         """Blocks until the results of a ``step_host(..., sync=False)`` are in the host buffers."""
-        _capi.check(self._L.mapdn_wait(self._h, torch.cuda.current_stream(self.device).cuda_stream))
+        _capi.check(self._L.mapdn_wait(self._h, self._stream()), self._L)
 
     def _compact_layout(self):
         if getattr(self, "_obs_slices", None) is None:
             off = (C.c_int32 * self.n_agents)()
             ln = (C.c_int32 * self.n_agents)()
             row = C.c_int32(0)
-            _capi.check(self._L.mapdn_obs_compact_layout(self._h, off, ln, C.byref(row)))
+            _capi.check(self._L.mapdn_obs_compact_layout(self._h, off, ln, C.byref(row)), self._L)
             self._obs_slices = [(int(off[a]), int(ln[a])) for a in range(self.n_agents)]
             self._obs_row_len = int(row.value)
         return self._obs_slices, self._obs_row_len
@@ -435,21 +447,21 @@ class BatchedVoltageControl:
         if self.history <= 1:
             return self.obs
         out = torch.empty_like(self.obs_stacked)
-        _capi.check(self._L.mapdn_get_obs_stacked(self._h, _ptr(out), self._stream()))
+        _capi.check(self._L.mapdn_get_obs_stacked(self._h, _ptr(out), self._stream()), self._L)
         return out
 
     # ---- getters ------------------------------------------------------------------------------
     def get_obs(self) -> torch.Tensor:
-        _capi.check(self._L.mapdn_get_obs(self._h, _ptr(self.obs), self._stream()))
+        _capi.check(self._L.mapdn_get_obs(self._h, _ptr(self.obs), self._stream()), self._L)
         return self.obs
 
     def get_state(self) -> torch.Tensor:
-        _capi.check(self._L.mapdn_get_state(self._h, _ptr(self.state), self._stream()))
+        _capi.check(self._L.mapdn_get_state(self._h, _ptr(self.state), self._stream()), self._L)
         return self.state
 
     def get_field(self, name: str) -> torch.Tensor:
         out = torch.empty(self.batch, self.dims.get(_capi.FIELD_DIMS.get(name), 1), dtype=torch.float64, device=self.device)
-        _capi.check(self._L.mapdn_get_field(self._h, _capi.FIELDS[name], _ptr(out), self._stream()))
+        _capi.check(self._L.mapdn_get_field(self._h, _capi.FIELDS[name], _ptr(out), self._stream()), self._L)
         return out
 
     # ---- env state snapshots (mapdn_snapshot / mapdn_restore) ----------------------------------------
@@ -466,7 +478,7 @@ class BatchedVoltageControl:
         """Byte offsets of the ``MAPDN_N_SNAPSHOT`` segments of a snapshot row, then bytes_per_env."""
         if self._snapshot_layout is None:
             off = (C.c_int64 * (len(_capi.SNAPSHOT_SEGMENTS) + 1))()
-            _capi.check(self._L.mapdn_snapshot_layout(self._h, off))
+            _capi.check(self._L.mapdn_snapshot_layout(self._h, off), self._L)
             self._snapshot_layout = [int(x) for x in off]
         return self._snapshot_layout
 
@@ -492,7 +504,7 @@ class BatchedVoltageControl:
         slots = torch.arange(self.batch) if idx is None else self._slots(idx, "snapshot", unique=False)
         data = torch.empty(slots.numel(), L[-1], dtype=torch.uint8, device=self.device)
         ids = None if idx is None else slots.to(self.device, torch.int32)
-        _capi.check(self._L.mapdn_snapshot(self._h, _ptr(ids), slots.numel(), _ptr(data), self._stream()))
+        _capi.check(self._L.mapdn_snapshot(self._h, _ptr(ids), slots.numel(), _ptr(data), self._stream()), self._L)
         return EnvSnapshot(data, slots + self.env_id_offset, L, self.history, self.fingerprint)
 
     def restore(self, snap: EnvSnapshot, idx=None) -> torch.Tensor:
@@ -524,11 +536,11 @@ class BatchedVoltageControl:
         whole = slots.numel() == self.batch and bool(torch.equal(slots, torch.arange(self.batch)))
         ids = None if whole else slots.to(self.device, torch.int32)
         st = self._stream()
-        _capi.check(self._L.mapdn_restore(self._h, _ptr(ids), slots.numel(), _ptr(data), st))
-        _capi.check(self._L.mapdn_get_obs(self._h, _ptr(self.obs), st))
-        _capi.check(self._L.mapdn_get_state(self._h, _ptr(self.state), st))
+        _capi.check(self._L.mapdn_restore(self._h, _ptr(ids), slots.numel(), _ptr(data), st), self._L)
+        _capi.check(self._L.mapdn_get_obs(self._h, _ptr(self.obs), st), self._L)
+        _capi.check(self._L.mapdn_get_state(self._h, _ptr(self.state), st), self._L)
         if self.history > 1:
-            _capi.check(self._L.mapdn_get_obs_stacked(self._h, _ptr(self.obs_stacked), st))
+            _capi.check(self._L.mapdn_get_obs_stacked(self._h, _ptr(self.obs_stacked), st), self._L)
         return slots
 
     def fork(self, src, dst) -> torch.Tensor:
@@ -544,7 +556,7 @@ class BatchedVoltageControl:
         (``RECORD_KEYS``: pv_active, pv_reactive, bus_active, bus_reactive, bus_voltage, line_loss)."""
         if getattr(self, "_record_slices", None) is None:
             off, row = (C.c_int32 * len(_capi.RECORD_KEYS))(), C.c_int32(0)
-            _capi.check(self._L.mapdn_record_layout(self._h, off, C.byref(row)))
+            _capi.check(self._L.mapdn_record_layout(self._h, off, C.byref(row)), self._L)
             ends = [int(o) for o in off][1:] + [int(row.value)]
             self._record_slices = {k: (int(o), e - int(o)) for k, o, e in zip(_capi.RECORD_KEYS, off, ends)}
             self._record_len = int(row.value)
@@ -566,7 +578,7 @@ class BatchedVoltageControl:
     def record(self, out: torch.Tensor) -> torch.Tensor:
         """The current tester record row of every env into ``out`` (``[B, record_len]`` view, any row stride): one gather
         launch. After a step, :meth:`step` with ``record=`` writes the same rows without it."""
-        _capi.check(self._L.mapdn_record(self._h, out.data_ptr(), self._record_stride(out), self._stream()))
+        _capi.check(self._L.mapdn_record(self._h, out.data_ptr(), self._record_stride(out), self._stream()), self._L)
         return out
 
     def get_avail_actions(self) -> torch.Tensor:
@@ -594,13 +606,14 @@ class BatchedVoltageControl:
         out["converged"] = torch.empty(nb, dtype=torch.uint8, device=self.device)
         _capi.check(self._L.mapdn_solve(self._h, nb, *[_ptr(t) for t in ins], _ptr(out["vm"]), _ptr(out["va_deg"]),
                                         _ptr(out["p_bus"]), _ptr(out["q_bus"]), _ptr(out["pl"]),
-                                        _ptr(out["iterations"]), _ptr(out["converged"]), self._stream()))
+                                        _ptr(out["iterations"]), _ptr(out["converged"]), self._stream()), self._L)
         return out
 
     def ybus_dense(self) -> np.ndarray:
         n = self.dims["n_bus"]
         g, b = np.zeros((n, n)), np.zeros((n, n))
-        _capi.check(self._L.mapdn_get_ybus_dense(self._h, g.ctypes.data_as(C.c_void_p), b.ctypes.data_as(C.c_void_p)))
+        _capi.check(self._L.mapdn_get_ybus_dense(self._h, g.ctypes.data_as(C.c_void_p), b.ctypes.data_as(C.c_void_p)),
+                    self._L)
         return g + 1j * b
 
 

@@ -13,34 +13,32 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 OUT = "/tmp/mapdn_emu_tsan"
 LIB = os.path.join(OUT, "libemu_tsan.so")
 CHILD = r'''
-import sys, numpy as np
+import sys, numpy as np, torch
 sys.path.insert(0, %(root)r); sys.path.insert(0, %(root)r + "/tests/emu")
 import emu_env
 emu_env.LIB = %(lib)r; emu_env.build = lambda force=False: emu_env.LIB
-from emu_env import EmuEnv
-from mapdn_b200 import cases
+from mapdn_b200 import baselines, cases
 name, lanes, B = sys.argv[1], int(sys.argv[2]), int(sys.argv[3])
 net, prof = cases.make_case(name), cases.make_profiles(name, n_days=3)
 scale = cases.SCENARIOS[name]["action_scale"]
-env = EmuEnv(net, prof, dict(seed=3, voltage_barrier_type="bowl", action_scale=scale), batch=B, lanes_per_env=lanes)
+env = emu_env.make_env(net, prof, dict(seed=3, voltage_barrier_type="bowl", action_scale=scale), batch=B, lanes_per_env=lanes)
 env.reset()
 rng = np.random.default_rng(0)
 for t in range(2):
-    env.step(rng.uniform(-scale, scale, (B, net.n_sgen)))
-env.step_host(rng.uniform(-scale, scale, (B, net.n_sgen)), path="compact")
+    env.step(torch.from_numpy(rng.uniform(-scale, scale, (B, net.n_sgen))))
+env.step_host(rng.uniform(-scale, scale, (B, net.n_sgen)), layout="compact")
 inp = cases.synthetic_inputs(name, 3, seed=1)
 env.solve(inp["p_load"], inp["q_load"], inp["p_pv"], np.zeros_like(inp["p_pv"]))
-env.droop(inp["p_load"], inp["q_load"], inp["p_pv"], inp["s_max"], max_ite=6)
+baselines.droop_control(env, inp["p_load"], inp["q_load"], inp["p_pv"], inp["s_max"], max_ite=6)
 print("ran", name, lanes, B)
 '''
 # auto-reset leg: episodes of 3 steps, half the batch reset early (terminated and running envs in one warp), one env per
 # step diverging, >= 2 persistent rounds (MAPDN_EMU_SMS / MAPDN_EPB from the caller)
 CHILD_AR = r'''
-import sys, numpy as np
+import sys, numpy as np, torch
 sys.path.insert(0, %(root)r); sys.path.insert(0, %(root)r + "/tests/emu")
 import emu_env
 emu_env.LIB = %(lib)r; emu_env.build = lambda force=False: emu_env.LIB
-from emu_env import EmuEnv, _ptr
 from mapdn_b200 import cases
 from mapdn_b200.network import ProfileDesc
 name, lanes, B, H = sys.argv[1], int(sys.argv[2]), int(sys.argv[3]), int(sys.argv[4])
@@ -48,23 +46,16 @@ net, prof = cases.make_case(name), cases.make_profiles(name, n_days=3)
 lp = prof.load_p.copy(); lp[60:460] *= 3000.0 if name == "case322" else 60.0
 prof = ProfileDesc(pv=prof.pv, load_p=lp, load_q=prof.load_q, steps_per_hour=prof.steps_per_hour, n_days=prof.n_days)
 scale = cases.SCENARIOS[name]["action_scale"]
-env = EmuEnv(net, prof, dict(seed=3, voltage_barrier_type="bowl", action_scale=scale, episode_limit=3), batch=B, lanes_per_env=lanes)
-L = emu_env.lib()
-if H > 1:
-    assert L.mapdn_set_history(env._h, H) == 0
+env = emu_env.make_env(net, prof, dict(seed=3, voltage_barrier_type="bowl", action_scale=scale, episode_limit=3, history=H),
+                       batch=B, lanes_per_env=lanes)
 env.reset()
-start = np.tile(np.array([[1, 5, 3]], np.int32), (B, 1)); start[1] = (0, 2, 18)
-env.reset(start, mask=(np.arange(B) %% 2).astype(np.uint8))
+start = torch.tensor([[1, 5, 3]] * B, dtype=torch.int32); start[1] = torch.tensor((0, 2, 18))
+env.reset(start, mask=torch.from_numpy((np.arange(B) %% 2).astype(np.uint8)))
 d = env.dims
-robs, ok = np.zeros((B, d["n_agents"], d["obs_dim"])), np.zeros(B, np.uint8)
-stk = np.zeros((B, d["n_agents"], H * d["obs_dim"])) if H > 1 else None
-rstk = np.zeros_like(stk) if H > 1 else None
 rng = np.random.default_rng(0)
 for t in range(5):
-    a = rng.uniform(-scale, scale, (B, net.n_sgen))
-    assert L.mapdn_step_autoreset(env._h, _ptr(a), 1, _ptr(env.reward), _ptr(env.term), _ptr(env.info), _ptr(env.obs),
-                                  _ptr(stk), _ptr(robs), _ptr(rstk), _ptr(ok), None) == 0
-rounds = -(-(-(-B // d["envs_per_block"])) // env.last_grid())
+    env.step_autoreset(torch.from_numpy(rng.uniform(-scale, scale, (B, net.n_sgen))))
+rounds = -(-(-(-B // d["envs_per_block"])) // emu_env.last_grid())
 print("ran", name, lanes, B, "rounds", rounds)
 '''
 

@@ -11,7 +11,8 @@ import os
 
 import numpy as np
 
-from mapdn_b200.network import NetDesc
+from mapdn_b200 import cases
+from mapdn_b200.network import NetDesc, ProfileDesc
 from oracle.voltage_control_ref import INFO_KEYS, VoltageControlOracle
 
 TOL = 1e-9            # reward, info, obs, vm, record rows
@@ -19,6 +20,52 @@ TOL_STATE = 1e-8      # state (bus p / q in MW, va in degrees)
 FIELDS = ("vm", "va_deg", "p_bus", "q_bus", "p_sgen", "q_sgen", "line_loss", "p_load", "q_load", "sum_rewards", "steps",
           "start_row", "nr_iters")
 RECORD_FIELDS = ("p_sgen", "q_sgen", "p_bus", "q_bus", "vm", "line_loss")   # the tester record row, block by block
+OVERRIDES = ("MAPDN_PLAN", "MAPDN_EPB", "MAPDN_HELPERS", "MAPDN_EMU_SMS")   # the planner's overrides, emulated SM count
+
+
+def set_geometry(monkeypatch, geom):
+    """Exactly the overrides in ``geom`` for the handles created next."""
+    for k in OVERRIDES:
+        monkeypatch.delenv(k, raising=False)
+    for k, v in geom.items():
+        monkeypatch.setenv(k, str(v))
+
+
+def same(a, b, exact, what, equal_nan=False):
+    """Bit for bit when ``exact``, else within 1e-10. ``equal_nan``: NaN where both have it (a sentinel of rows a call must
+    not write) counts as equal; without it any NaN fails."""
+    if exact:
+        assert np.array_equal(a, b, equal_nan=equal_nan), what
+    elif equal_nan:
+        assert a.shape == b.shape and np.array_equal(np.isnan(a), np.isnan(b)), what
+        d = np.abs(np.nan_to_num(a) - np.nan_to_num(b))
+        assert d.size == 0 or d.max() <= 1e-10, (what, float(d.max()))
+    else:
+        assert a.shape == b.shape and np.abs(a - b).max() <= 1e-10, (what, float(np.abs(a - b).max()))
+
+
+def overload(net, prof, factor=60.0):
+    """The profile with rows 60..459 carrying a demand the feeder cannot serve (the divergence branch of step)."""
+    lp = prof.load_p.copy(); lp[60:460] *= factor
+    return net, ProfileDesc(pv=prof.pv, load_p=lp, load_q=prof.load_q, steps_per_hour=prof.steps_per_hour, n_days=prof.n_days)
+
+
+def overloaded_case(name, n_days=4):
+    """A named case through :func:`overload` (case322's synthetic demand is light: 60 times of it can still be served)."""
+    return overload(cases.make_case(name), cases.make_profiles(name, n_days=n_days), 3000.0 if name == "case322" else 60.0)
+
+
+def mesh4():
+    """A meshed 4-bus net (the dense fallback solver) with a random four-day profile."""
+    z = np.array([0.02 + 0.04j, 0.01 + 0.03j, 0.0125 + 0.025j, 0.015 + 0.03j])
+    net = NetDesc(base_mva=100.0, n_bus=4, slack_bus=0, slack_vm=1.03, br_from=np.array([0, 0, 1, 2]), br_to=np.array([1, 2, 2, 3]),
+                  br_r=z.real, br_x=z.imag, load_bus=np.array([1, 2, 3]), sgen_bus=np.array([2, 3]), sgen_zone=np.array([1, 1]),
+                  bus_zone=np.array([0, 1, 1, 1]), name="mesh4")
+    rng = np.random.default_rng(3)
+    T = 4 * 24 * 20 + 1
+    prof = ProfileDesc(pv=rng.uniform(0, 40, (T, 2)), load_p=rng.uniform(60, 180, (T, 3)), load_q=rng.uniform(10, 60, (T, 3)),
+                       steps_per_hour=20)
+    return net, prof
 
 
 def actions(batch, n_sgen, scale, n_steps, seed):

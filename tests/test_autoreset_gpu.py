@@ -13,8 +13,8 @@ from mapdn_b200 import cases
 from mapdn_b200.env import BatchedVoltageControl
 from mapdn_b200.marl_runner import BatchedMarlRunner, DeviceTransitionBuffer
 from mapdn_b200.rollout import BatchedRollout, DeviceReplayBuffer
-from test_history_emu import _overload
-from test_history_gpu import FIELDS, _Recorder
+from geometry_cases import FIELDS, overloaded_case
+from test_history_gpu import _Recorder
 
 pytestmark = pytest.mark.gpu
 
@@ -31,7 +31,7 @@ def _same(a, b, exact, what):
 @pytest.mark.parametrize("H", [1, 3])
 @pytest.mark.parametrize("name,batch", [("case33", 4096), ("case141", 2048), ("case322", 1024), ("case322", 512)])
 def test_benchmark_sizes_autoreset_equals_step_then_reset(name, batch, H):
-    net, prof = _overload(cases.make_case(name), cases.make_profiles(name, n_days=4), 3000.0 if name == "case322" else 60.0)
+    net, prof = overloaded_case(name)
     args = dict(voltage_barrier_type="l1", seed=7, action_scale=cases.SCENARIOS[name]["action_scale"], episode_limit=4,
                 history=H)
     A = BatchedVoltageControl(net, prof, args, batch=batch)
@@ -96,7 +96,7 @@ class _NoAutoReset:
 
 
 def _env(H):
-    net, prof = _overload(cases.make_case("case33"), cases.make_profiles("case33", n_days=6))
+    net, prof = overloaded_case("case33", n_days=6)
     args = dict(voltage_barrier_type="l1", seed=4, action_scale=0.8, episode_limit=3, history=H)
     return BatchedVoltageControl(net, prof, args, batch=64)
 

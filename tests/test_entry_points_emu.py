@@ -21,7 +21,7 @@ from mapdn_b200.env import DEFAULT_ENV_ARGS
 from mapdn_b200.network import NetDesc
 
 sys.path.insert(0, os.path.join(ROOT, "tests", "emu"))
-from emu_env import EmuEnv, lib                                     # noqa: E402
+from emu_env import lib, make_env                                   # noqa: E402
 
 INVALID = 1
 NULL_ARG, NO_PROFILE = "null argument", "handle was created without a profile store"
@@ -43,7 +43,7 @@ STEPS = {
 @pytest.fixture(scope="module")
 def envs():
     net, prof = cases.make_case("case33"), cases.make_profiles("case33", n_days=3)
-    env, bare = EmuEnv(net, prof, dict(voltage_barrier_type="l1"), batch=B), EmuEnv(net, None, dict(voltage_barrier_type="l1"), batch=B)
+    env, bare = make_env(net, prof, dict(voltage_barrier_type="l1"), batch=B), make_env(net, None, dict(voltage_barrier_type="l1"), batch=B)
     env.reset()
     d = env.dims
     ng, row = d["n_sgen"], 2 * d["n_sgen"] + 3 * d["n_bus"] + d["n_line"]
@@ -205,6 +205,6 @@ def test_create_refusals(case):
 
 
 def test_create_launches_the_two_ybus_kernels():
-    env = EmuEnv(cases.make_case("case33"), None, batch=B)
-    assert lib().mapdn_launch_count(env._h) == 2
+    env = make_env(cases.make_case("case33"), None, batch=B)
+    assert env.launch_count == 2
     env.close()

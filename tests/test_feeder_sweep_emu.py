@@ -6,7 +6,6 @@ Two fp64 implementations of the same Newton iteration legitimately drift apart w
 the mp reference the kernel must be as accurate as the oracle itself: |V - V_mp| <= C_ORACLE * |V_oracle - V_mp| + 1e-12,
 besides the absolute bound. Results need not be bit-identical across lane counts: the schedules change the order in
 which children are accumulated."""
-import ctypes as C
 import multiprocessing as mp
 import os
 import sys
@@ -22,7 +21,7 @@ from oracle.mp_newton import MpNewton
 from oracle.pandapower_nr import PandapowerEquivalent, make_ybus
 
 sys.path.insert(0, os.path.join(ROOT, "tests", "emu"))
-from emu_env import EmuEnv, lib                                      # noqa: E402
+from emu_env import make_env, nan_filled_outputs                    # noqa: E402,F401  (autouse fixture)
 
 from feeder_cases import LANES, TOL_NR, check_env, refusal_bytes   # noqa: E402
 
@@ -30,6 +29,10 @@ UNSUPPORTED = 4
 
 NETS = FC.catalogue("emu")
 MESHED = FC.meshed_catalogue()
+
+
+def _solve(env, *inputs):
+    return {k: v.numpy() for k, v in env.solve(*inputs).items()}
 
 
 def _reference(item):
@@ -57,13 +60,13 @@ def test_generated_feeder_matches_mp_newton_at_every_lane_count(name, references
     live = [k for k in range(len(rmp)) if not rmp[k].ambiguous(TOL_NR)]
     for lanes in LANES:
         try:
-            env = EmuEnv(net, None, dict(voltage_barrier_type="l1"), batch=1, lanes_per_env=lanes)
+            env = make_env(net, None, dict(voltage_barrier_type="l1"), batch=1, lanes_per_env=lanes)
         except RuntimeError as ex:       # an explicit lane count may not fit; the default always must
             need, _, avail = refusal_bytes(str(ex))
             assert lanes != 0 and need > avail, (name, lanes)
             continue
         try:
-            out = env.solve(*inp)
+            out = _solve(env, *inp)
         finally:
             env.close()
         for k in live:
@@ -75,9 +78,9 @@ def test_generated_meshed_feeder_matches_mp_newton(name, references):
     """The dense fallback (one warp per env whatever lanes_per_env asks)."""
     net = MESHED[name]
     inp, rmp, ror = references[name]
-    env = EmuEnv(net, None, dict(voltage_barrier_type="l1"), batch=1)
+    env = make_env(net, None, dict(voltage_barrier_type="l1"), batch=1)
     assert env.dims["lanes_per_env"] == 32
-    out = env.solve(*inp)
+    out = _solve(env, *inp)
     env.close()
     for k in range(len(rmp)):
         if not rmp[k].ambiguous(TOL_NR):
@@ -94,20 +97,13 @@ def test_generated_cases_span_the_loading_range_and_are_rarely_ambiguous(referen
     assert sum(not r.converged for r in rs) >= 0.05 * len(rs)
 
 
-def _ybus_dense(env):
-    n = env.dims["n_bus"]
-    g, b = np.zeros((n, n)), np.zeros((n, n))
-    env._chk(lib().mapdn_get_ybus_dense(env._h, C.c_void_p(g.ctypes.data), C.c_void_p(b.ctypes.data)))
-    return g + 1j * b
-
-
 @pytest.mark.parametrize("name", ["random40", "decades4", "hub4", "forest12"])
 def test_device_ybus_with_phase_shifters_matches_makeYbus(name):
     """ybus_branch_kernel / ybus_diag_kernel with shifters: Ybus is asymmetric, and Y[i,j] vs Y[j,i] must land right."""
     net = NETS[name]
     assert np.any(net.br_shift != 0)
-    env = EmuEnv(net, None, dict(voltage_barrier_type="l1"), batch=1)
-    Y, Yo = _ybus_dense(env), make_ybus(net)[0].toarray()
+    env = make_env(net, None, dict(voltage_barrier_type="l1"), batch=1)
+    Y, Yo = env.ybus_dense(), make_ybus(net)[0].toarray()
     env.close()
     assert np.abs(Yo - Yo.T).max() > 1e-3 * np.abs(Yo).max()
     assert np.abs(Y - Yo).max() <= 1e-12 * np.abs(Yo).max()
@@ -143,7 +139,7 @@ def test_default_lane_count_of_accepted_nets_is_unchanged():
     nets = [cases.make_case(c) for c in ("case33", "case141", "case322")] + [random_tree_net(23, 4, seed=11)]
     nets += [S.SCENARIOS[s]["build"]()[0] for s in sorted(S.SCENARIOS)]
     for net in nets:
-        env = EmuEnv(net, None, dict(voltage_barrier_type="l1"), batch=4)
+        env = make_env(net, None, dict(voltage_barrier_type="l1"), batch=4)
         assert env.dims["lanes_per_env"] == _default_lanes(net.n_bus - 1), net.name
         env.close()
 
@@ -161,12 +157,12 @@ def test_default_lane_count_falls_back_for_a_deep_feeder():
                   br_r=rng.uniform(1e-4, 4e-4, n - 1), br_x=rng.uniform(1e-4, 4e-4, n - 1), load_bus=np.arange(1, n),
                   sgen_bus=[n - 1, n // 2], sgen_zone=[1, 1], bus_zone=[0] + [1] * (n - 1), name="chain400")
     with pytest.raises(RuntimeError, match="too large"):
-        EmuEnv(net, None, None, batch=1, lanes_per_env=64).close()
-    env = EmuEnv(net, None, dict(voltage_barrier_type="l1"), batch=1, lanes_per_env=0)
+        make_env(net, None, None, batch=1, lanes_per_env=64).close()
+    env = make_env(net, None, dict(voltage_barrier_type="l1"), batch=1, lanes_per_env=0)
     assert env.dims["lanes_per_env"] in (4, 8, 16, 32)
     pl = rng.uniform(0.0, 2e-3, (2, net.n_load)) * np.array([[1.0], [4.0]])
     inp = (pl, 0.3 * pl, np.full((2, net.n_sgen), 1e-3), np.zeros((2, net.n_sgen)))
-    out = env.solve(*inp)
+    out = _solve(env, *inp)
     env.close()
     m, pf = MpNewton(net), PandapowerEquivalent(net)
     for k in range(2):
@@ -181,7 +177,7 @@ def test_refusal_states_the_bytes_the_smallest_plan_needs(lanes):
     """A net no plan fits: the message names a byte count above the opt-in limit it was refused against."""
     n = 400 if lanes else 1700
     with pytest.raises(RuntimeError) as ex:
-        EmuEnv(_chain(n), None, None, batch=1, lanes_per_env=lanes)
+        make_env(_chain(n), None, None, batch=1, lanes_per_env=lanes)
     msg = str(ex.value)
     assert f"mapdn status {UNSUPPORTED}" in msg
     need, at, avail = refusal_bytes(msg)
@@ -192,4 +188,4 @@ def test_refusal_states_the_bytes_the_smallest_plan_needs(lanes):
 def test_a_bus_with_258_children_is_refused(lanes):
     net = FC.feeder(FC.hub(258), seed=5, name="hub258")
     with pytest.raises(RuntimeError, match=f"mapdn status {UNSUPPORTED}: a bus with more than 257 children"):
-        EmuEnv(net, None, None, batch=1, lanes_per_env=lanes)
+        make_env(net, None, None, batch=1, lanes_per_env=lanes)

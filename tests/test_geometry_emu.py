@@ -16,20 +16,18 @@ import sys
 
 import numpy as np
 import pytest
+import torch
 
 import geometry_cases as GC
 from conftest import ROOT, random_tree_net
-from mapdn_b200 import cases
+from mapdn_b200 import baselines, cases
 from mapdn_b200.network import NetDesc, ProfileDesc
 
 sys.path.insert(0, os.path.join(ROOT, "tests", "emu"))
-from emu_env import EmuEnv                                          # noqa: E402
+from emu_env import last_grid, make_env, nan_filled_outputs          # noqa: E402,F401  (autouse fixture)
 from oracle.pandapower_nr import PandapowerEquivalent               # noqa: E402
 from oracle.voltage_control_ref import INFO_KEYS, VoltageControlOracle   # noqa: E402
 from test_emu_kernel import _oracle_droop                           # noqa: E402
-
-OVERRIDES = ("MAPDN_PLAN", "MAPDN_EPB", "MAPDN_HELPERS", "MAPDN_EMU_SMS")
-
 
 def _random_profile(net, seed, pv_hi, load_hi):
     rng = np.random.default_rng(seed)
@@ -71,14 +69,6 @@ def _rounds(batch, epb, grid):
     return -(-needed // grid)
 
 
-def _set_geometry(monkeypatch, geom):
-    for k in OVERRIDES:
-        monkeypatch.delenv(k, raising=False)
-    for k, v in geom.items():
-        if k in OVERRIDES:
-            monkeypatch.setenv(k, str(v))
-
-
 def _solve_inputs(net, prof, batch, seed):
     rng = np.random.default_rng(seed)
     rows = rng.integers(0, prof.n_rows, batch)
@@ -90,44 +80,44 @@ def _solve_inputs(net, prof, batch, seed):
 def run_geometry(monkeypatch, name, lanes, batch, geom, n_steps=2, seed=5, droop=True):
     """One trajectory on one geometry; returns (dims, grids, trajectory, solve, droop) - all of it, for the comparisons."""
     net, prof, scale = _net(name)
-    _set_geometry(monkeypatch, geom)
+    GC.set_geometry(monkeypatch, geom)
     args = dict(voltage_barrier_type="bowl", action_scale=scale, seed=seed)
-    env = EmuEnv(net, prof, args, batch=batch, lanes_per_env=lanes, env_id_offset=100)
+    env = make_env(net, prof, args, batch=batch, lanes_per_env=lanes, env_id_offset=100)
     try:
         acts = GC.actions(batch, net.n_sgen, scale, n_steps, seed)
-        _, R = env.record_layout()
-        rec = np.full((batch, n_steps + 1, R), np.nan)
+        R = env.record_len
+        rec = torch.full((batch, n_steps + 1, R), np.nan, dtype=torch.float64)
         out = {k: [] for k in ("obs", "state", "iters", "reward", "term", "info")}
         fields = {k: [] for k in GC.FIELDS}
         grids = []
 
         def snap():
-            out["obs"].append(env.obs.copy()); out["state"].append(env.get_state().copy())
+            out["obs"].append(env.obs.numpy().copy()); out["state"].append(env.get_state().numpy().copy())
             for k in GC.FIELDS:
-                fields[k].append(env.get_field(k))
+                fields[k].append(env.get_field(k).numpy())
             out["iters"].append(fields["nr_iters"][-1][:, 0].astype(np.int64))
         env.reset_ok[:] = 7
         env.reset()
-        grids.append(env.last_grid())
-        reset_ok = env.reset_ok.copy()
+        grids.append(last_grid())
+        reset_ok = env.reset_ok.numpy().copy()
         env.record(rec[:, 0])
         snap()
         for t in range(n_steps):
-            r, tm, info = env.step_record(acts[t], rec[:, t + 1])
-            grids.append(env.last_grid())
-            out["reward"].append(r.copy()); out["term"].append(tm.copy()); out["info"].append(info.copy())
+            r, tm, info = [x.numpy().copy() for x in env.step(torch.from_numpy(acts[t]), record=rec[:, t + 1])]
+            grids.append(last_grid())
+            out["reward"].append(r); out["term"].append(tm); out["info"].append(info)
             snap()
         traj = {k: np.array(v) for k, v in out.items()}
-        traj["rec"] = rec.transpose(1, 0, 2).copy()
+        traj["rec"] = rec.numpy().transpose(1, 0, 2).copy()
         traj["fields"] = {k: np.array(v) for k, v in fields.items()}
         traj["reset_ok"] = reset_ok
         ins = _solve_inputs(net, prof, batch, seed)
-        sol = env.solve(*ins)
-        grids.append(env.last_grid())
+        sol = {k: v.numpy() for k, v in env.solve(*ins).items()}
+        grids.append(last_grid())
         dr = None
         if droop:
-            dr = env.droop(ins[0], ins[1], ins[2], prof.s_max)
-            grids.append(env.last_grid())
+            dr = {k: v.numpy() for k, v in baselines.droop_control(env, ins[0], ins[1], ins[2], prof.s_max).items()}
+            grids.append(last_grid())
         return dict(dims=env.dims, grids=grids, traj=traj, solve=sol, droop=dr, ins=ins, net=net, prof=prof, args=env.args,
                     acts=acts)
     finally:
@@ -251,13 +241,6 @@ def test_geometry_matrix_is_bit_identical_and_matches_the_oracle(monkeypatch, gr
     _assert_plans(spec, smem_of)
 
 
-def _overload(name):
-    """The named case with a profile whose rows 60..459 carry a demand the feeder cannot serve."""
-    net, prof = cases.make_case(name), cases.make_profiles(name, n_days=3)
-    lp = prof.load_p.copy(); lp[60:460] *= 60.0
-    return net, ProfileDesc(pv=prof.pv, load_p=lp, load_q=prof.load_q, steps_per_hour=prof.steps_per_hour, n_days=prof.n_days)
-
-
 @pytest.mark.parametrize("geom,want", [(dict(MAPDN_EMU_SMS=1), (32, 7, 182560, 1, 2)),
                                        (dict(MAPDN_EMU_SMS=1, MAPDN_PLAN=3, MAPDN_EPB=4, MAPDN_HELPERS=4), (32, 4, 98928, 2, 2))])
 def test_diverging_and_never_converging_envs_in_later_rounds(monkeypatch, geom, want):
@@ -266,14 +249,15 @@ def test_diverging_and_never_converging_envs_in_later_rounds(monkeypatch, geom, 
     diverge: reset_ok reports it for env 13 only, the other envs are untouched bit for bit and env 13 keeps its power
     flow results. Every other env matches the oracle throughout (env 13 until its failed reset: the reference retries
     such a reset for ever), and both geometries give the same bits, env 13 included."""
-    net, prof = _overload("case141")
+    net, prof = GC.overload(cases.make_case("case141"), cases.make_profiles("case141", n_days=3))
     B, scale = 14, cases.SCENARIOS["case141"]["action_scale"]
     args = dict(voltage_barrier_type="l1", action_scale=scale, seed=9)
     start = np.array([[1, e % 24, (3 * e) % 20] for e in range(B)], np.int32)       # day 1: clear of the overload
     start[11] = (0, 2, 18)                         # row 58: the reset solves row 59, step 1 loads row 60, step 2 diverges
-    _set_geometry(monkeypatch, geom)
-    env = EmuEnv(net, prof, args, batch=B, env_id_offset=100)
+    GC.set_geometry(monkeypatch, geom)
+    env = make_env(net, prof, args, batch=B, env_id_offset=100)
     d = env.dims
+    obs, reset_ok = env.obs.numpy(), env.reset_ok.numpy()
     ors = [VoltageControlOracle(net, prof, env.args, env_id=100 + e) for e in range(B)]
     acts = GC.actions(B, net.n_sgen, scale, 4, seed=2)
     trace = []
@@ -281,15 +265,15 @@ def test_diverging_and_never_converging_envs_in_later_rounds(monkeypatch, geom, 
     live = list(range(B))
 
     def compare(label):
-        st = env.get_state()
+        st = env.get_state().numpy()
         for e in live:
             o = ors[e]
-            assert np.abs(np.array(o.get_obs()) - env.obs[e]).max() < GC.TOL, (label, e)
+            assert np.abs(np.array(o.get_obs()) - obs[e]).max() < GC.TOL, (label, e)
             assert np.abs(o.get_state() - st[e]).max() < GC.TOL_STATE, (label, e)
-        trace.append((env.obs.copy(), st.copy(), np.concatenate([env.get_field(k) for k in GC.FIELDS], axis=1)))
+        trace.append((obs.copy(), st.copy(), np.concatenate([env.get_field(k).numpy() for k in GC.FIELDS], axis=1)))
 
-    env.reset(start)
-    grid = env.last_grid()
+    env.reset(torch.from_numpy(start))
+    grid = last_grid()
     assert (d["lanes_per_env"], d["envs_per_block"], d["smem_bytes"], grid, _rounds(B, d["envs_per_block"], grid)) == want
     assert -(-12 // d["envs_per_block"]) > grid                     # env 11 runs in round 2
     for e, o in enumerate(ors):
@@ -300,20 +284,20 @@ def test_diverging_and_never_converging_envs_in_later_rounds(monkeypatch, geom, 
         if t == 2:
             mask = np.zeros(B, np.uint8); mask[13] = 1
             st2 = start.copy(); st2[13] = (0, 5, 0)                  # row 100: every draw diverges
-            before = {k: env.get_field(k) for k in GC.FIELDS}
-            b_obs, b_state = env.obs.copy(), env.get_state().copy()
+            before = {k: env.get_field(k).numpy() for k in GC.FIELDS}
+            b_obs, b_state = obs.copy(), env.get_state().numpy().copy()
             env.reset_ok[:] = 7
-            env.reset(st2, mask=mask)
-            assert env.reset_ok[13] == 0 and np.all(env.reset_ok[:13] == 7)
-            assert np.array_equal(env.obs[:13], b_obs[:13]) and np.array_equal(env.get_state()[:13], b_state[:13])
+            env.reset(torch.from_numpy(st2), mask=torch.from_numpy(mask))
+            assert reset_ok[13] == 0 and np.all(reset_ok[:13] == 7)
+            assert np.array_equal(obs[:13], b_obs[:13]) and np.array_equal(env.get_state().numpy()[:13], b_state[:13])
             for k in GC.FIELDS:
-                after = env.get_field(k)
+                after = env.get_field(k).numpy()
                 assert np.array_equal(after[:13], before[k][:13]), k
                 if k in ("vm", "va_deg", "p_bus", "q_bus", "line_loss"):
                     assert np.array_equal(after[13], before[k][13]), k
             live.remove(13)
-        r, term, info = env.step(acts[t])
-        it = env.get_field("nr_iters")[:, 0]
+        r, term, info = [x.numpy() for x in env.step(torch.from_numpy(acts[t]))]
+        it = env.get_field("nr_iters").numpy()[:, 0]
         trace.append((r.copy(), term.copy(), info.copy()))
         for e in live:
             o = ors[e]
@@ -348,12 +332,12 @@ def test_meshed_case141_dense_fallback_matches_the_oracle(monkeypatch):
 
 def test_meshed_net_size_limit_of_the_dense_fallback(monkeypatch):
     """256 PQ buses are accepted (one warp per env, 2 npq = 512); 257 are refused at create with MAPDN_ERR_TOPOLOGY (3)."""
-    _set_geometry(monkeypatch, dict(MAPDN_EMU_SMS=1))
-    env = EmuEnv(GC.meshed_chain(256), None, dict(voltage_barrier_type="l1"), batch=1)
+    GC.set_geometry(monkeypatch, dict(MAPDN_EMU_SMS=1))
+    env = make_env(GC.meshed_chain(256), None, dict(voltage_barrier_type="l1"), batch=1)
     assert env.dims["lanes_per_env"] == 32 and env.dims["n_bus"] == 257
     env.close()
     with pytest.raises(RuntimeError, match=r"mapdn status 3: .*more than 256 PQ buses"):
-        EmuEnv(GC.meshed_chain(257), None, dict(voltage_barrier_type="l1"), batch=1)
+        make_env(GC.meshed_chain(257), None, dict(voltage_barrier_type="l1"), batch=1)
 
 
 @pytest.mark.parametrize("lanes,cap", [(32, 8), (64, 8), (128, 4)])
@@ -361,7 +345,7 @@ def test_envs_per_block_override_is_capped(monkeypatch, lanes, cap):
     """MAPDN_EPB cannot exceed the solver threads the planner's own search allows (256 for G <= 32, 512 above: the
     kernel's launch bounds and the named-barrier ids 3 + group): a small net whose shared memory would allow more."""
     net, prof, _ = _net("hub")
-    _set_geometry(monkeypatch, dict(MAPDN_EPB=64))
-    env = EmuEnv(net, prof, None, batch=64, lanes_per_env=lanes)
+    GC.set_geometry(monkeypatch, dict(MAPDN_EPB=64))
+    env = make_env(net, prof, None, batch=64, lanes_per_env=lanes)
     assert env.dims["lanes_per_env"] == lanes and env.dims["envs_per_block"] == cap
     env.close()

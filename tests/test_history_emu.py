@@ -12,59 +12,17 @@ import sys
 
 import numpy as np
 import pytest
+import torch
 
+import geometry_cases as GC
 from conftest import ROOT
 from mapdn_b200 import cases
-from mapdn_b200.network import ProfileDesc
 from oracle import ref_scenarios as S
 
 sys.path.insert(0, os.path.join(ROOT, "tests", "emu"))
-import emu_env                                                       # noqa: E402
-from emu_env import EmuEnv, _ptr                                     # noqa: E402
+from emu_env import last_grid, make_env, nan_filled_outputs          # noqa: E402,F401  (autouse fixture)
 
-FIELDS = ("vm", "va_deg", "p_bus", "q_bus", "p_sgen", "q_sgen", "line_loss", "p_load", "q_load", "sum_rewards", "steps",
-          "start_row", "nr_iters")
-
-
-def _lib():
-    return emu_env.lib()
-
-
-def _overload(net, prof, factor=60.0):
-    """The profile with rows 60..459 carrying a demand the feeder cannot serve (the divergence branch of step)."""
-    lp = prof.load_p.copy(); lp[60:460] *= factor
-    return net, ProfileDesc(pv=prof.pv, load_p=lp, load_q=prof.load_q, steps_per_hour=prof.steps_per_hour, n_days=prof.n_days)
-
-
-def _mesh():
-    from mapdn_b200.network import NetDesc
-    z = np.array([0.02 + 0.04j, 0.01 + 0.03j, 0.0125 + 0.025j, 0.015 + 0.03j])
-    net = NetDesc(base_mva=100.0, n_bus=4, slack_bus=0, slack_vm=1.03, br_from=np.array([0, 0, 1, 2]), br_to=np.array([1, 2, 2, 3]),
-                  br_r=z.real, br_x=z.imag, load_bus=np.array([1, 2, 3]), sgen_bus=np.array([2, 3]), sgen_zone=np.array([1, 1]),
-                  bus_zone=np.array([0, 1, 1, 1]), name="mesh4")
-    rng = np.random.default_rng(3)
-    T = 4 * 24 * 20 + 1
-    prof = ProfileDesc(pv=rng.uniform(0, 40, (T, 2)), load_p=rng.uniform(60, 180, (T, 3)), load_q=rng.uniform(10, 60, (T, 3)),
-                       steps_per_hour=20)
-    return net, prof
-
-
-def set_history(env, H):
-    return _lib().mapdn_set_history(env._h, H)
-
-
-def step_stacked(env, a, stacked, obs=True, rec=None, add_noise=True):
-    """mapdn_step_stacked on an EmuEnv; returns the status."""
-    a = np.ascontiguousarray(a, np.float64)
-    return _lib().mapdn_step_stacked(env._h, _ptr(a), int(add_noise), _ptr(env.reward), _ptr(env.term), _ptr(env.info),
-                                     _ptr(env.obs) if obs else None, _ptr(stacked), _ptr(rec),
-                                     0 if rec is None else rec.strides[0] // 8, None)
-
-
-def get_stacked(env, H):
-    out = np.full((env.batch, env.dims["n_agents"], H * env.dims["obs_dim"]), np.nan)
-    env._chk(_lib().mapdn_get_obs_stacked(env._h, _ptr(out), None))
-    return out
+NAN = float("nan")
 
 
 def stacking_rule(frames, H):
@@ -77,42 +35,29 @@ def stacking_rule(frames, H):
     return np.stack(rows)
 
 
-def _same(a, b, exact, what):
-    if exact:
-        assert np.array_equal(a, b), what
-    else:
-        assert a.shape == b.shape and np.abs(a - b).max() <= 1e-10, (what, float(np.abs(a - b).max()))
-
-
-def _set_geometry(monkeypatch, geom):
-    for k in ("MAPDN_PLAN", "MAPDN_EPB", "MAPDN_HELPERS", "MAPDN_EMU_SMS"):
-        monkeypatch.delenv(k, raising=False)
-    for k, v in geom.items():
-        monkeypatch.setenv(k, str(v))
-
-
 # step paths of the handle with history, cycled; the history = 1 handle always takes mapdn_step_record with obs
 KINDS = ("stacked", "record", "pinned", "no_obs", "f32", "plain")
 
 
 def run_history(monkeypatch, net, prof, args, batch, lanes, H, geom, diverge_env):
-    _set_geometry(monkeypatch, geom)
-    plain = EmuEnv(net, prof, args, batch=batch, lanes_per_env=lanes)
-    hist = EmuEnv(net, prof, args, batch=batch, lanes_per_env=lanes)
-    assert set_history(hist, H) == 0
+    GC.set_geometry(monkeypatch, geom)
+    plain = make_env(net, prof, args, batch=batch, lanes_per_env=lanes)
+    hist = make_env(net, prof, dict(args, history=H), batch=batch, lanes_per_env=lanes)
     d = hist.dims
     exact = d["lanes_per_env"] <= 32
     grid_rounds = []
     ng, od = d["n_agents"], d["obs_dim"]
-    _, R = hist.record_layout()
+    R = hist.record_len
     B = batch
+    p_obs, h_obs, stacked = plain.obs.numpy(), hist.obs.numpy(), hist.obs_stacked.numpy()
 
-    plain.reset(None, add_noise=True); hist.reset(None, add_noise=True)
-    _same(plain.obs, hist.obs, exact, "reset obs")
-    frames = [[plain.obs[b].copy()] for b in range(B)]
-    got = get_stacked(hist, H)
-    assert np.array_equal(got, stacking_rule(frames, H))
-    assert np.all(got[:, :, :(H - 1) * od] == 0.0)                   # before the episode start: exactly zero
+    plain.reset(None, add_noise=True)
+    hist.obs_stacked[:] = NAN
+    hist.reset(None, add_noise=True)
+    GC.same(p_obs, h_obs, exact, "reset obs")
+    frames = [[p_obs[b].copy()] for b in range(B)]
+    assert np.array_equal(stacked, stacking_rule(frames, H))
+    assert np.all(stacked[:, :, :(H - 1) * od] == 0.0)               # before the episode start: exactly zero
 
     rng = np.random.default_rng(H + 10 * d["lanes_per_env"])
     scale = float(args.get("action_scale", 0.8))
@@ -124,48 +69,54 @@ def run_history(monkeypatch, net, prof, args, batch, lanes, H, geom, diverge_env
     diverged = False
     for t in range(n_steps):
         if t == mid:
-            plain.reset(start, add_noise=True, mask=mask); hist.reset(start, add_noise=True, mask=mask)
-            assert np.array_equal(plain.reset_ok[mask == 1], hist.reset_ok[mask == 1]) and hist.reset_ok[mask == 1].all()
-            _same(plain.obs[mask == 1], hist.obs[mask == 1], exact, "masked reset obs")
+            plain.reset(torch.from_numpy(start), add_noise=True, mask=torch.from_numpy(mask))
+            hist.obs_stacked[:] = NAN
+            hist.reset(torch.from_numpy(start), add_noise=True, mask=torch.from_numpy(mask))
+            p_ok, h_ok = plain.reset_ok.numpy(), hist.reset_ok.numpy()
+            assert np.array_equal(p_ok[mask == 1], h_ok[mask == 1]) and h_ok[mask == 1].all()
+            GC.same(p_obs[mask == 1], h_obs[mask == 1], exact, "masked reset obs")
             for b in np.nonzero(mask)[0]:
-                frames[b] = [plain.obs[b].copy()]
-            got = get_stacked(hist, H)
-            assert np.array_equal(got, stacking_rule(frames, H))
-            assert np.all(got[mask == 1][:, :, :(H - 1) * od] == 0.0)
+                frames[b] = [p_obs[b].copy()]
+            assert np.array_equal(stacked, stacking_rule(frames, H))
+            assert np.all(stacked[mask == 1][:, :, :(H - 1) * od] == 0.0)
         kind = KINDS[t % len(KINDS)]
-        a = rng.uniform(-scale, scale, (B, ng))
-        rec0, rec1 = np.full((B, R + 2), np.nan), np.full((B, R + 2), np.nan)
-        r0, t0, i0 = [x.copy() for x in plain.step_record(a, rec0[:, :R])]
-        stacked = np.full((B, ng, H * od), np.nan)
+        a = torch.from_numpy(rng.uniform(-scale, scale, (B, ng)))
+        rec0, rec1 = torch.full((B, R + 2), NAN, dtype=torch.float64), torch.full((B, R + 2), NAN, dtype=torch.float64)
+        r0, t0, i0 = [x.numpy().copy() for x in plain.step(a, record=rec0[:, :R])]
+        hist.obs_stacked[:] = NAN
         if kind in ("stacked", "record", "no_obs"):
-            hist.obs[:] = np.nan
-            st = step_stacked(hist, a, None if kind == "no_obs" else stacked, obs=kind != "no_obs",
-                              rec=rec1[:, :R] if kind == "record" else None)
-            assert st == 0, _lib().mapdn_last_error()
-            r1, t1, i1, o1 = hist.reward.copy(), hist.term.copy(), hist.info.copy(), hist.obs.copy()
-        elif kind == "plain":
-            r1, t1, i1 = [x.copy() for x in hist.step(a)]
-            o1 = hist.obs.copy()
+            hist.obs[:] = NAN
+            r1, t1, i1 = [x.numpy().copy() for x in hist.step(a, want_obs=kind != "no_obs",
+                                                             record=rec1[:, :R] if kind == "record" else None)]
+            o1 = h_obs.copy()
+        elif kind == "plain":                           # mapdn_step on a handle with history: the ring still records
+            L = hist._L
+            assert L.mapdn_step(hist._h, a.data_ptr(), 1, hist.reward.data_ptr(), hist.terminated.data_ptr(),
+                                hist.info.data_ptr(), hist.obs.data_ptr(), None) == 0, L.mapdn_last_error()
+            r1, t1, i1, o1 = hist.reward.numpy().copy(), hist.terminated.numpy().copy(), hist.info.numpy().copy(), h_obs.copy()
         else:
-            r1, t1, i1, o1 = hist.step_host(a, f32=kind == "f32", path="pinned" if kind == "pinned" else "staged")
-        grid_rounds.append(-(-(-(-B // d["envs_per_block"])) // hist.last_grid()))     # rounds of this step's launch
-        _same(r0, r1, exact, (kind, t, "reward")); assert np.array_equal(t0, t1), (kind, t)
-        _same(i0, i1, exact, (kind, t, "info"))
+            host = hist._host_buffers()                 # padded host rows: the pinned path never writes the padding
+            host["obs"].zero_(); host["obs32"][:] = NAN
+            r1, t1, i1, o1 = hist.step_host(a.numpy(), obs_dtype=np.float32 if kind == "f32" else np.float64,
+                                            staged=kind == "f32")
+        grid_rounds.append(-(-(-(-B // d["envs_per_block"])) // last_grid()))     # rounds of this step's launch
+        GC.same(r0, r1, exact, (kind, t, "reward")); assert np.array_equal(t0, t1), (kind, t)
+        GC.same(i0, i1, exact, (kind, t, "info"))
         if kind == "f32":
-            assert np.array_equal(plain.obs.astype(np.float32), o1) if exact else np.abs(plain.obs - o1).max() < 1e-5
+            assert np.array_equal(p_obs.astype(np.float32), o1) if exact else np.abs(p_obs - o1).max() < 1e-5
         elif kind != "no_obs":
-            _same(plain.obs, o1, exact, (kind, t, "obs"))
+            GC.same(p_obs, o1, exact, (kind, t, "obs"))
         else:
-            assert np.all(np.isnan(o1))                                        # nothing written
+            assert np.all(np.isnan(o1)) and np.all(np.isnan(stacked))              # nothing written
         if kind == "record":
-            _same(rec0[:, :R], rec1[:, :R], exact, (t, "record")); assert np.all(np.isnan(rec1[:, R:]))
-        for k in FIELDS:
-            _same(plain.get_field(k), hist.get_field(k), exact, (kind, t, k))
-        _same(plain.get_state(), hist.get_state(), exact, (kind, t, "state"))
+            GC.same(rec0[:, :R].numpy(), rec1[:, :R].numpy(), exact, (t, "record")); assert torch.all(rec1[:, R:].isnan())
+        for k in GC.FIELDS:
+            GC.same(plain.get_field(k).numpy(), hist.get_field(k).numpy(), exact, (kind, t, k))
+        GC.same(plain.get_state().numpy(), hist.get_state().numpy(), exact, (kind, t, "state"))
         for b in range(B):
-            frames[b].append(plain.obs[b].copy())
+            frames[b].append(p_obs[b].copy())
         want = stacking_rule(frames, H)
-        got = get_stacked(hist, H)
+        got = hist.get_obs_stacked().numpy()
         # the ring holds the padded fp64 frames of the history handle's own launches: exact against them
         if exact:
             assert np.array_equal(got, want), (kind, t)
@@ -180,14 +131,9 @@ def run_history(monkeypatch, net, prof, args, batch, lanes, H, geom, diverge_env
     return d
 
 
-def _case(name):
-    # case322's synthetic demand is light: 60 times of it can still be served
-    return _overload(cases.make_case(name), cases.make_profiles(name, n_days=4), 3000.0 if name == "case322" else 60.0)
-
-
 @pytest.mark.parametrize("H", [2, 3, 5])
 def test_case33_stacked_rows(monkeypatch, H):
-    net, prof = _case("case33")
+    net, prof = GC.overloaded_case("case33")
     d = run_history(monkeypatch, net, prof, dict(voltage_barrier_type="l1", seed=3, action_scale=0.8), batch=24, lanes=0,
                     H=H, geom=dict(MAPDN_EMU_SMS=1, MAPDN_EPB=20), diverge_env=5)
     assert d["lanes_per_env"] == 8
@@ -195,7 +141,7 @@ def test_case33_stacked_rows(monkeypatch, H):
 
 @pytest.mark.parametrize("name,lanes,batch,epb", [("case141", 32, 9, 4), ("case322", 64, 4, 3), ("case322", 128, 3, 2)])
 def test_large_feeders_stacked_rows(monkeypatch, name, lanes, batch, epb):
-    net, prof = _case(name)
+    net, prof = GC.overloaded_case(name)
     d = run_history(monkeypatch, net, prof, dict(voltage_barrier_type="bowl", seed=4,
                                                  action_scale=cases.SCENARIOS[name]["action_scale"]),
                     batch=batch, lanes=lanes, H=3, geom=dict(MAPDN_EMU_SMS=1, MAPDN_EPB=epb), diverge_env=1)
@@ -203,7 +149,7 @@ def test_large_feeders_stacked_rows(monkeypatch, name, lanes, batch, epb):
 
 
 def test_dense_meshed_fallback_stacked_rows(monkeypatch):
-    net, prof = _overload(*_mesh())
+    net, prof = GC.overload(*GC.mesh4())
     run_history(monkeypatch, net, prof, dict(voltage_barrier_type="l2", seed=2, episode_limit=48), batch=5, lanes=0, H=3,
                 geom=dict(MAPDN_EMU_SMS=1, MAPDN_EPB=2), diverge_env=1)
 
@@ -233,73 +179,86 @@ def test_reference_history_fixture_on_the_emulation():
     sc = S.SCENARIOS["case33_history"]
     net, prof = sc["build"]()
     H = sc["args"]["history"]
-    env = EmuEnv(net, prof, sc["args"], batch=1)
-    assert set_history(env, H) == 0
-    assert g["obs"].shape[-1] == H * env.dims["obs_dim"]
+    env = make_env(net, prof, sc["args"], batch=1)
+    assert env.history == H and g["obs"].shape[-1] == H * env.dims["obs_dim"]
     want = reference_rows_one_frame_per_transition(g, ops, H, env.dims["obs_dim"])
     t = 0
     for k_op, op in enumerate(ops):
+        env.obs_stacked[:] = NAN
         if op[0] == "step":
-            stacked = np.full((1, net.n_sgen, H * env.dims["obs_dim"]), np.nan)
-            assert step_stacked(env, g["actions"][t], stacked, add_noise=op[1]) == 0
-            assert np.array_equal(stacked, get_stacked(env, H))
+            env.step(torch.from_numpy(np.asarray(g["actions"][t], np.float64).reshape(1, net.n_sgen)), add_noise=bool(op[1]))
+            assert np.array_equal(env.obs_stacked.numpy(), env.get_obs_stacked().numpy())
             t += 1
         else:
             assert op[0] in ("init", "reset")
             env.reset()
-        assert np.abs(get_stacked(env, H)[0] - want[k_op]).max() < 1e-9, (k_op, op)
+        assert np.abs(env.get_obs_stacked().numpy()[0] - want[k_op]).max() < 1e-9, (k_op, op)
+        assert np.abs(env.obs_stacked.numpy()[0] - want[k_op]).max() < 1e-9, (k_op, op)
     env.close()
 
 
 def test_refusals_and_the_history_lifecycle():
     """Refusals leave the launch count alone; H = 1 frees the ring, H > 1 (again) records from the next reset on; a reset
-    of a handle with history is two launches (the reset, frame 0 into the ring), a step one."""
-    L = _lib()
+    of a handle with history is two launches (the reset, frame 0 into the ring), a step one. The history is set on the
+    handle directly (mapdn_set_history), so the ring's entry points are called directly too."""
     net, prof = cases.make_case("case33"), cases.make_profiles("case33", n_days=4)
-    env = EmuEnv(net, prof, dict(seed=1), batch=3)
+    env = make_env(net, prof, dict(seed=1), batch=3)
+    L, h = env._L, env._h
     od, ng, B = env.dims["obs_dim"], net.n_sgen, 3
-    a = np.zeros((B, ng))
-    buf = np.zeros((B, 5 * ng * od))
-    n = L.mapdn_launch_count(env._h)
+    a = torch.zeros(B, ng, dtype=torch.float64)
+    buf = torch.zeros(B, 5 * ng * od, dtype=torch.float64)
+    n = L.mapdn_launch_count(h)
+
+    def step_stacked(out, rec=None):
+        return L.mapdn_step_stacked(h, a.data_ptr(), 1, env.reward.data_ptr(), env.terminated.data_ptr(), env.info.data_ptr(),
+                                    env.obs.data_ptr(), out.data_ptr(), None if rec is None else rec.data_ptr(),
+                                    0 if rec is None else rec.stride(0), None)
+
+    def gather(H):
+        out = torch.full((B, ng, H * od), NAN, dtype=torch.float64)
+        assert L.mapdn_get_obs_stacked(h, out.data_ptr(), None) == 0, L.mapdn_last_error()
+        return out.numpy()
 
     def refused(st, text):
         assert st == 1 and text in L.mapdn_last_error().decode(), L.mapdn_last_error()
-        assert L.mapdn_launch_count(env._h) == n
+        assert L.mapdn_launch_count(h) == n
 
     refused(L.mapdn_set_history(None, 3), "null handle")
-    refused(set_history(env, 0), "history must be >= 1")
-    refused(set_history(env, -2), "history must be >= 1")
-    refused(step_stacked(env, a, buf), "no observation history")
-    refused(L.mapdn_get_obs_stacked(env._h, _ptr(buf), None), "no observation history")
-    refused(L.mapdn_get_obs_stacked(None, _ptr(buf), None), "null argument")
-    refused(L.mapdn_step_stacked(None, _ptr(a), 1, _ptr(env.reward), _ptr(env.term), None, None, None, None, 0, None), "null argument")
-    assert set_history(env, 3) == 0
-    rec = np.zeros((B, 4))
-    refused(step_stacked(env, a, buf, rec=rec), "record_stride")
-    refused(L.mapdn_get_obs_stacked(env._h, None, None), "null argument")
+    refused(L.mapdn_set_history(h, 0), "history must be >= 1")
+    refused(L.mapdn_set_history(h, -2), "history must be >= 1")
+    refused(step_stacked(buf), "no observation history")
+    refused(L.mapdn_get_obs_stacked(h, buf.data_ptr(), None), "no observation history")
+    refused(L.mapdn_get_obs_stacked(None, buf.data_ptr(), None), "null argument")
+    refused(L.mapdn_step_stacked(None, a.data_ptr(), 1, env.reward.data_ptr(), env.terminated.data_ptr(), None, None, None,
+                                 None, 0, None), "null argument")
+    assert L.mapdn_set_history(h, 3) == 0
+    rec = torch.zeros(B, 4, dtype=torch.float64)
+    refused(step_stacked(buf, rec=rec), "record_stride")
+    refused(L.mapdn_get_obs_stacked(h, None, None), "null argument")
 
     frames = None
+    obs = env.obs.numpy()
     for H in (3, 1, 2):
-        assert set_history(env, H) == 0
+        assert L.mapdn_set_history(h, H) == 0
         env.reset()
-        n = L.mapdn_launch_count(env._h)
+        n = L.mapdn_launch_count(h)
         if H == 1:
-            refused(step_stacked(env, a, buf), "no observation history")
+            refused(step_stacked(buf), "no observation history")
             env.step(a)
-            assert L.mapdn_launch_count(env._h) == n + 1
+            assert L.mapdn_launch_count(h) == n + 1
             continue
-        frames = [[env.obs[b].copy()] for b in range(B)]
-        assert np.array_equal(get_stacked(env, H), stacking_rule(frames, H))
-        n = L.mapdn_launch_count(env._h)
+        frames = [[obs[b].copy()] for b in range(B)]
+        assert np.array_equal(gather(H), stacking_rule(frames, H))
+        n = L.mapdn_launch_count(h)
         for _ in range(H + 1):
-            st = np.zeros((B, ng, H * od))
-            assert step_stacked(env, a, st) == 0
+            st = torch.zeros(B, ng, H * od, dtype=torch.float64)
+            assert step_stacked(st) == 0
             for b in range(B):
-                frames[b].append(env.obs[b].copy())
-            assert np.array_equal(st, stacking_rule(frames, H))
-        assert L.mapdn_launch_count(env._h) == n + H + 1
-        env.reset(mask=np.array([0, 1, 0], np.uint8))
-        assert L.mapdn_launch_count(env._h) == n + H + 3
-        frames[1] = [env.obs[1].copy()]
-        assert np.array_equal(get_stacked(env, H), stacking_rule(frames, H))
+                frames[b].append(obs[b].copy())
+            assert np.array_equal(st.numpy(), stacking_rule(frames, H))
+        assert L.mapdn_launch_count(h) == n + H + 1
+        env.reset(mask=torch.tensor([0, 1, 0], dtype=torch.uint8), want_state=False)
+        assert L.mapdn_launch_count(h) == n + H + 3
+        frames[1] = [obs[1].copy()]
+        assert np.array_equal(gather(H), stacking_rule(frames, H))
     env.close()

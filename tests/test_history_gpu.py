@@ -9,15 +9,13 @@ import pytest
 import torch
 
 from conftest import ROOT
+from geometry_cases import FIELDS
 from mapdn_b200 import cases
 from mapdn_b200.env import BatchedVoltageControl
 from mapdn_b200.marl_runner import BatchedMarlRunner, BatchedPolicyTester
 from oracle import ref_scenarios as S
 
 pytestmark = pytest.mark.gpu
-
-FIELDS = ("vm", "va_deg", "p_bus", "q_bus", "p_sgen", "q_sgen", "line_loss", "p_load", "q_load", "sum_rewards", "steps",
-          "start_row", "nr_iters")
 
 
 def stacking_rule(frames, H):

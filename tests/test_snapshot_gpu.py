@@ -13,12 +13,9 @@ from mapdn_b200 import cases
 from mapdn_b200.env import BatchedVoltageControl, EnvSnapshot
 from mapdn_b200.marl_runner import BatchedMarlRunner, DeviceTransitionBuffer, attach
 from mapdn_b200.rollout import BatchedRollout, DeviceReplayBuffer
-from test_history_emu import _overload
+from geometry_cases import FIELDS, overloaded_case
 
 pytestmark = pytest.mark.gpu
-
-FIELDS = ("vm", "va_deg", "p_bus", "q_bus", "p_sgen", "q_sgen", "line_loss", "p_load", "q_load", "sum_rewards", "steps",
-          "start_row", "nr_iters")
 
 
 def _eq(a, b, what):
@@ -44,7 +41,7 @@ def _getters(env):
 
 
 def _env(name, batch, H, offset=0, **kw):
-    net, prof = _overload(cases.make_case(name), cases.make_profiles(name, n_days=4), 3000.0 if name == "case322" else 60.0)
+    net, prof = overloaded_case(name)
     args = dict(voltage_barrier_type="l1", seed=7, action_scale=cases.SCENARIOS[name]["action_scale"], episode_limit=4,
                 history=H)
     return BatchedVoltageControl(net, prof, args, batch=batch, env_id_offset=offset, **kw)

@@ -1,5 +1,6 @@
-"""Host logic of env state snapshots, without a GPU: the fingerprint, placement of snapshot rows by global env id, the
-checkpoint format, and BatchedRollout resuming on a CPU stand-in env that implements snapshot / restore."""
+"""Host logic of env state snapshots, without a GPU: the fingerprint, placement of snapshot rows by global env id (on the
+CPU emulation of the library, tests/emu), the checkpoint format, and BatchedRollout resuming on a CPU stand-in env that
+implements snapshot / restore."""
 import ctypes as C
 import os
 import subprocess
@@ -15,6 +16,9 @@ from mapdn_b200.env import BatchedVoltageControl, EnvSnapshot, snapshot_fingerpr
 from mapdn_b200.network import ProfileDesc
 from mapdn_b200.rollout import BatchedRollout, DeviceReplayBuffer
 from test_autoreset_rollout_cpu import _AutoResetEnv
+
+sys.path.insert(0, os.path.join(ROOT, "tests", "emu"))
+from emu_env import make_env                                        # noqa: E402
 
 ARGS = dict(voltage_barrier_type="bowl", voltage_weight=1.0, q_weight=0.1, line_weight=None, v_upper=1.05, v_lower=0.95,
             episode_limit=240, action_scale=0.8, action_bias=0.0, reset_action=True, seed=3,
@@ -58,7 +62,56 @@ def test_fingerprint_fills_in_the_solver_defaults():
     assert _fp(tol=1e-8, max_iter=10) == _fp()
 
 
-# ---- placement by global id, on a handle whose library calls are recorded ------------------------------------------------
+# ---- placement by global id, on the emulated library ----------------------------------------------------------------------
+def _emu(batch, offset=0, history=1):
+    """A case33 handle of the CPU emulation of the kernel source (tests/emu), its envs reset and stepped once."""
+    env = make_env(cases.make_case("case33"), cases.make_profiles("case33", n_days=3), dict(ARGS, history=history),
+                   batch=batch, env_id_offset=offset, lanes_per_env=8)
+    env.reset()
+    env.step(torch.from_numpy(np.random.default_rng(batch + offset).uniform(-0.8, 0.8, (batch, env.n_agents))))
+    return env
+
+
+def _rows_of(env, gather=True):
+    """The snapshot rows, and obs / state / obs_stacked: gathered now, or (gather=False) as the env's buffers hold them
+    (restore gathers them again for all envs)."""
+    if gather:
+        out = dict(obs=env.get_obs().clone(), state=env.get_state().clone(), obs_stacked=env.get_obs_stacked().clone())
+    else:
+        out = dict(obs=env.obs.clone(), state=env.state.clone(), obs_stacked=env.obs_stacked.clone())
+    out["rows"] = env.snapshot().data.clone()
+    return out
+
+
+def test_restore_places_rows_by_global_id():
+    for H in (1, 3):
+        src = _emu(12, history=H)
+        snap, want = src.snapshot(range(8)), _rows_of(src)            # global ids 0..7
+        for offset in (0, 4):
+            env = _emu(4, offset, history=H)
+            assert env.restore(snap).tolist() == [0, 1, 2, 3]
+            got = _rows_of(env, gather=False)
+            for k in want:
+                assert torch.equal(got[k], want[k][offset:offset + 4]), (H, offset, k)
+        env = _emu(6, 5, history=H)                                    # ids 5..10: rows 5..7 of the snapshot
+        before = _rows_of(env)
+        assert env.restore(snap).tolist() == [0, 1, 2]
+        got = _rows_of(env, gather=False)
+        for k in want:
+            assert torch.equal(got[k][:3], want[k][5:8]) and torch.equal(got[k][3:], before[k][3:]), (H, k)
+    env = _emu(4, 100)
+    rows, n = env.snapshot().data, env.launch_count
+    assert env.restore(_emu(4).snapshot()).numel() == 0               # no id of this handle: nothing launched
+    assert env.launch_count == n and torch.equal(env.snapshot().data, rows)
+    env = _emu(4, 0)
+    src = _emu(4, 0)
+    before, want = _rows_of(env), _rows_of(src)
+    env.restore(src.snapshot([3, 1]), idx=[0, 2])                      # explicit slots
+    got = _rows_of(env, gather=False)
+    for k in want:
+        assert torch.equal(got[k][[0, 2]], want[k][[3, 1]]) and torch.equal(got[k][[1, 3]], before[k][[1, 3]]), k
+
+
 class _RecordingLib:
     """mapdn_restore / the gathers of a handle, recorded instead of launched (pointers are CPU tensors' addresses)."""
 
@@ -67,76 +120,57 @@ class _RecordingLib:
 
     def mapdn_restore(self, h, idx, n, buf, stream):
         ids = None if idx is None else list((C.c_int32 * n).from_address(idx.value))
-        rows = np.frombuffer(C.string_at(buf.value, n * self.bpe), np.uint8).reshape(n, self.bpe).copy()
-        self.calls.append(("restore", ids, rows))
+        self.calls.append(("restore", ids))
         return 0
 
     def mapdn_get_obs(self, *a):
-        self.calls.append(("get_obs",)); return 0
+        return 0
 
     def mapdn_get_state(self, *a):
-        self.calls.append(("get_state",)); return 0
-
-    def mapdn_get_obs_stacked(self, *a):
-        self.calls.append(("get_obs_stacked",)); return 0
+        return 0
 
 
-def _handle(batch, offset, history=1, bpe=32):
+def test_no_index_list_when_all_envs_are_in_order():
+    """Every slot in order goes to mapdn_restore without an index list; anything else with one."""
     env = BatchedVoltageControl.__new__(BatchedVoltageControl)
-    env.batch, env.env_id_offset, env.history = batch, offset, history
+    env.batch, env.env_id_offset, env.history, env._cpu = 4, 4, 1, True
     env.device = torch.device("cpu")
-    env._h, env._L = C.c_void_p(1), _RecordingLib(bpe)
-    env._snapshot_layout, env._fingerprint = [0] * 15 + [bpe], "fp"
+    env._h, env._L = C.c_void_p(1), _RecordingLib(32)
+    env._snapshot_layout, env._fingerprint = [0] * 15 + [32], "fp"
     env.obs = env.state = env.obs_stacked = torch.zeros(1)
-    env._stream = lambda: None
-    return env
+    env.restore(_snap(range(8)))
+    env.restore(_snap([0, 1]), idx=[3, 1])
+    assert env._L.calls == [("restore", None), ("restore", [3, 1])]
+
+
+def test_restore_refusals():
+    env = _emu(4, 0)
+    one, two = env.snapshot([1]), env.snapshot([1, 2])
+    n = env.launch_count
+    with pytest.raises(ValueError, match="duplicate"):
+        env.restore(two, idx=[3, 3])
+    with pytest.raises(ValueError, match="slots must be in"):
+        env.restore(two, idx=[0, 4])
+    with pytest.raises(ValueError, match="2 slots for 1"):
+        env.restore(one, idx=[0, 1])
+    with pytest.raises(ValueError, match="duplicate"):
+        env.restore(env.snapshot([1, 1]))                              # two rows for one global id
+    n = env.launch_count
+    wider = EnvSnapshot(torch.zeros(1, one.layout[-1] + 16, dtype=torch.uint8), one.env_ids, one.layout[:-1] + [one.layout[-1] + 16],
+                        1, one.fingerprint)
+    with pytest.raises(ValueError, match="layout"):
+        env.restore(wider)
+    with pytest.raises(ValueError, match="layout"):
+        env.restore(EnvSnapshot(one.data, one.env_ids, one.layout, 2, one.fingerprint))
+    with pytest.raises(ValueError, match="another net"):
+        env.restore(EnvSnapshot(one.data, one.env_ids, one.layout, 1, "other"))
+    assert env.launch_count == n
 
 
 def _snap(ids, bpe=32, history=1):
     ids = torch.as_tensor(ids, dtype=torch.int64)
     data = (ids[:, None] * 3 + torch.arange(bpe)[None, :]).to(torch.uint8)
     return EnvSnapshot(data, ids, [0] * 15 + [bpe], history, "fp")
-
-
-def test_restore_places_rows_by_global_id():
-    snap = _snap(range(8))
-    for offset in (0, 4):
-        env = _handle(4, offset)
-        slots = env.restore(snap)
-        assert slots.tolist() == [0, 1, 2, 3]
-        kind, ids, rows = env._L.calls[0]
-        assert ids is None                                             # all envs in order: no index list
-        assert np.array_equal(rows, snap.data[offset:offset + 4].numpy())
-        assert [c[0] for c in env._L.calls[1:]] == ["get_obs", "get_state"]
-    env = _handle(6, 5, history=3)                                     # ids 5..10: rows 5..7 of the snapshot
-    slots = env.restore(_snap(range(8), history=3))
-    kind, ids, rows = env._L.calls[0]
-    assert slots.tolist() == [0, 1, 2] and ids == [0, 1, 2] and np.array_equal(rows, _snap(range(5, 8)).data.numpy())
-    assert env._L.calls[-1] == ("get_obs_stacked",)
-    assert _handle(4, 100).restore(snap).numel() == 0                  # no id of this handle: nothing launched
-    env = _handle(4, 0)
-    env.restore(_snap([3, 1]), idx=[0, 2])                             # explicit slots
-    assert env._L.calls[0][1] == [0, 2]
-
-
-def test_restore_refusals():
-    env = _handle(4, 0)
-    with pytest.raises(ValueError, match="duplicate"):
-        env.restore(_snap([1, 2]), idx=[3, 3])
-    with pytest.raises(ValueError, match="slots must be in"):
-        env.restore(_snap([1, 2]), idx=[0, 4])
-    with pytest.raises(ValueError, match="2 slots for 1"):
-        env.restore(_snap([1]), idx=[0, 1])
-    with pytest.raises(ValueError, match="duplicate"):
-        env.restore(_snap([1, 1]))                                     # two rows for one global id
-    with pytest.raises(ValueError, match="layout"):
-        env.restore(_snap([1], bpe=48))
-    with pytest.raises(ValueError, match="layout"):
-        env.restore(_snap([1], history=2))
-    bad = _snap([1]); bad.fingerprint = "other"
-    with pytest.raises(ValueError, match="another net"):
-        env.restore(bad)
-    assert env._L.calls == []
 
 
 def test_state_dict_loads_with_weights_only(tmp_path):
